@@ -927,3 +927,13 @@ void co_reset_many(CoEnv **envs, int n, uint8_t *obs) {
     if (obs) co_render(envs[i], obs + (size_t)i * envs[i]->sw * envs[i]->sh * 3);
   }
 }
+/* Row i of the output belongs to envs[i]: frames, semantic maps, player vectors (co_export_player). */
+void co_render_many(CoEnv **envs, int n, uint8_t *obs) {
+  for (int i = 0; i < n; ++i) co_render(envs[i], obs + (size_t)i * envs[i]->sw * envs[i]->sh * 3);
+}
+void co_semantic_many(CoEnv **envs, int n, uint8_t *out) {
+  for (int i = 0; i < n; ++i) co_semantic(envs[i], out + (size_t)i * envs[i]->aw * envs[i]->ah);
+}
+void co_export_player_many(CoEnv **envs, int n, int64_t *out) {
+  for (int i = 0; i < n; ++i) co_export_player(envs[i], out + (size_t)i * 49);
+}

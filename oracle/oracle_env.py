@@ -232,40 +232,80 @@ def world_seed(seed, episode):
 
 
 class OracleBatch:
-  """N oracle envs stepped by a thread pool (CPU baseline of bench.py; env i has seed0 + i)."""
+  """N oracle envs stepped by a thread pool (CPU baseline of bench.py, full-batch parity test; env i
+  has seed0 + i).  `threads` defaults to every host core.  Rendering is stateless (the night noise is
+  keyed by the step), so skipping it with render=False changes nothing but the time taken."""
 
-  def __init__(self, num_envs, threads, seed=0, **kwargs):
+  def __init__(self, num_envs, threads=None, seed=0, **kwargs):
     import concurrent.futures
+    import os
     self.envs = [OracleEnv(seed=seed + i, **kwargs) for i in range(num_envs)]
-    self.n, self.threads = num_envs, max(1, min(threads, num_envs))
-    self.size = self.envs[0].size
+    self.n, self.threads = num_envs, max(1, min(threads or os.cpu_count() or 1, num_envs))
+    self.size, self.area = self.envs[0].size, self.envs[0].area
     self.obs = np.zeros((num_envs, self.size[1], self.size[0], 3), np.uint8)
     self.reward = np.zeros(num_envs, np.float64)
     self.done = np.zeros(num_envs, np.int32)
     self._ptrs = (ctypes.c_void_p * num_envs)(*[e._h for e in self.envs])
     self._pool = concurrent.futures.ThreadPoolExecutor(self.threads)
-    bounds = np.linspace(0, num_envs, self.threads + 1).astype(int)
-    self._chunks = [(int(a), int(b)) for a, b in zip(bounds[:-1], bounds[1:]) if b > a]
+    self._chunks = self._split(num_envs)
     L = lib()
-    L.co_step_many.argtypes = [ctypes.c_void_p] * 5 + [ctypes.c_void_p, ctypes.c_int]
     L.co_step_many.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
                                ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
-    L.co_reset_many.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
+    for name in ('co_reset_many', 'co_render_many', 'co_semantic_many', 'co_export_player_many'):
+      getattr(L, name).argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
+
+  def _split(self, n):
+    bounds = np.linspace(0, n, min(self.threads, max(n, 1)) + 1).astype(int)
+    return [(int(a), int(b)) for a, b in zip(bounds[:-1], bounds[1:]) if b > a]
 
   def _ptr(self, a):
     return ctypes.addressof(self._ptrs) + a * ctypes.sizeof(ctypes.c_void_p)
 
-  def reset(self):
-    obs_stride = self.obs[0].nbytes
-    list(self._pool.map(lambda c: lib().co_reset_many(
-        self._ptr(c[0]), c[1] - c[0], self.obs.ctypes.data + c[0] * obs_stride), self._chunks))
+  def _map(self, fn, ids, out):
+    """fn(envs, n, out) over the envs `ids` (all when None) in parallel chunks; row k of `out`
+    belongs to env ids[k]."""
+    if ids is None:
+      ptrs, n = self._ptrs, self.n
+    else:
+      ids = np.asarray(ids, np.int64).reshape(-1)
+      ptrs, n = (ctypes.c_void_p * max(len(ids), 1))(*[self.envs[i]._h for i in ids]), len(ids)
+    addr, step = ctypes.addressof(ptrs), ctypes.sizeof(ctypes.c_void_p)
+    row = out[0].nbytes if out is not None and len(out) else 0
+    data = out.ctypes.data if out is not None else None
+    list(self._pool.map(lambda c: fn(addr + c[0] * step, c[1] - c[0],
+                                     None if data is None else data + c[0] * row), self._split(n)))
+    return out
+
+  def reset(self, ids=None, render=True):
+    """Start a new episode in every env (or in those of `ids`); with render, obs holds the frames."""
+    out = None
+    if render:
+      out = self.obs if ids is None else np.zeros((len(ids),) + self.obs.shape[1:], np.uint8)
+    self._map(lib().co_reset_many, ids, out)
+    if render and ids is not None:
+      self.obs[np.asarray(ids, np.int64)] = out
     return self.obs
 
-  def step(self, actions, auto_reset=True):
+  def step(self, actions, auto_reset=True, render=True):
     actions = np.ascontiguousarray(actions, np.int32)
     obs_stride = self.obs[0].nbytes
     list(self._pool.map(lambda c: lib().co_step_many(
         self._ptr(c[0]), c[1] - c[0], actions.ctypes.data + 4 * c[0],
         self.reward.ctypes.data + 8 * c[0], self.done.ctypes.data + 4 * c[0],
-        self.obs.ctypes.data + c[0] * obs_stride, int(auto_reset)), self._chunks))
+        self.obs.ctypes.data + c[0] * obs_stride if render else None, int(auto_reset)), self._chunks))
     return self.obs, self.reward, self.done.astype(bool)
+
+  def render(self, ids=None):
+    """Frames of the envs `ids` (all when None) as they stand: (len(ids), H, W, 3) uint8."""
+    n = self.n if ids is None else len(ids)
+    return self._map(lib().co_render_many, ids, np.zeros((n,) + self.obs.shape[1:], np.uint8))
+
+  def semantic(self, ids=None):
+    """info['semantic'] of the envs `ids` (all when None): (len(ids), W, H) uint8."""
+    n = self.n if ids is None else len(ids)
+    return self._map(lib().co_semantic_many, ids, np.zeros((n,) + tuple(self.area), np.uint8))
+
+  def player(self, ids=None):
+    """The 49-entry player vectors of oracle/canon.py of the envs `ids` (all when None): (len(ids), 49)."""
+    n = self.n if ids is None else len(ids)
+    return self._map(lib().co_export_player_many, ids, np.zeros((n, 49), np.int64))
