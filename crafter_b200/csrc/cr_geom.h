@@ -40,14 +40,18 @@ inline const char *geom_from_config(const cr_config &c, Geom &g) {
     g.tsz_magic = tsz > 1 ? (uint32_t)(((1ull << 32) + tsz - 1) / tsz) : 0u;
     g.tile_sq = tsz > 0 ? RENDER_NT / tsz : 0;
     g.tile_sr = tsz > 0 ? RENDER_NT % tsz : 0;
-    g.tile_cache = tsz <= 1024;  // 54 tiles x 4 KB; larger units (render(512)) go per pixel
+    g.tile_cache = tsz <= 1024;  // 54 tiles x 4 KB; larger units (render(512)) go per pixel, and so do
+                                 // units whose cache cr_create finds too large for the shared memory
   }
   g.seed = c.seed; g.env_offset = c.env_offset;
   g.obs_evict_first = 0;  // CRAFTER_B200_OBS_EVICT_FIRST
   g.draw_prefetch = 0;  // CRAFTER_B200_DRAW_PREFETCH
   g.incr_census = 0;    // CRAFTER_B200_INCR_CENSUS
-  if (g.gy < 1 || g.ux < 1 || g.uy < 1 || g.vw * g.vh > 256 || g.ux > 255 || g.uy > 255)
-    return "view/size not supported (need view_h > item rows, unit in 1..255, window <= 256 cells)";
+  // A unit of 1 pixel has no room for the item icons (0.8 * unit rounds to 0, env.py:240), and the tile
+  // cache's division by the unit size (tsz_magic) needs a unit of 2 texels or more.
+  if (g.ux < 2 || g.uy < 2) return "unit below 2 pixels: size must be at least twice the view on each axis";
+  if (g.gy < 1 || g.vw * g.vh > 256 || g.ux > 255 || g.uy > 255)
+    return "view/size not supported (need view_h > item rows, unit <= 255, window <= 256 cells)";
   if (g.CAP < 8 || g.CAP > 65535) return "slot_capacity must be in 8..65535";
   if (g.NCH * 5 * 2 > 40000) return "area too large (more than 4000 chunks)";
   if (g.W > 32767 || g.H > 32767) return "area side must fit int16";

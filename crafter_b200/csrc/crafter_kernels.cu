@@ -373,6 +373,9 @@ int create_on_device(cr_handle *h, const cr_config *c, const cr_tables *t, const
   CR_CUDA(raise_smem((const void *)k_post<true>, h->balance_smem));
   CR_CUDA(raise_smem((const void *)k_post<false>, h->balance_smem));
   const size_t tile = align16((size_t)g.sw * g.sh * 3);
+  // a tile cache that does not fit beside the frame's tables (a unit of 32 x 32 texels: 54 tiles of 4 KB,
+  // e.g. render(512) at view 16) is dropped: every cell per pixel
+  if (g.tile_cache && render_tile_offset(g) > (size_t)max_smem) g.tile_cache = 0;
   const size_t fixed = render_tile_offset(g);
   if (fixed > (size_t)max_smem) return fail_msg("unit too large for the tile cache");
   // keep at least two CTAs per SM when staging the output tile

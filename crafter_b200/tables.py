@@ -55,10 +55,15 @@ def _draw_alpha(canvas, pos, texture):
   canvas[x: x + w, y: y + h] = texture
 
 
+UNIT_TOO_SMALL = 'unit below 2 pixels: size must be at least twice the view on each axis'  # = cr_geom.h
+
+
 def geometry(view, size):
   view = np.array(view if hasattr(view, '__len__') else (view, view))
   size = np.array(size if hasattr(size, '__len__') else (size, size))
   unit = size // view  # env.py:122
+  if (unit < 2).any():  # the reference fails later, inside PIL (an item icon of 0.8 * unit = 0 pixels)
+    raise ValueError(UNIT_TOO_SMALL)
   item_rows = int(np.ceil(len(rules.ITEMS) / view[0]))  # env.py:42
   grid = np.array([view[0], view[1] - item_rows])  # env.py:43-44
   border = (size - unit * view) // 2  # env.py:127

@@ -104,11 +104,15 @@ static void render_one(hs_handle *h, int env, uint8_t *obs) {  // obs: the batch
   memcpy(obs + (size_t)env * bytes, tile.data(), bytes);
 }
 
+static const char *g_error = "";
+
 extern "C" {
+
+const char *hs_last_error() { return g_error; }
 
 int hs_create(const cr_config *c, const cr_tables *t, const cr_state *s, hs_handle **out) {
   hs_handle *h = new hs_handle();
-  if (geom_from_config(*c, h->g)) { delete h; return -2; }
+  if (const char *msg = geom_from_config(*c, h->g)) { g_error = msg; delete h; return -2; }
   state_from_abi(*s, h->st);
   h->rt.mat_tex = t->mat_tex; h->rt.obj_tex = t->obj_tex; h->rt.item_tile = t->item_tile;
   h->rt.vignette = t->vignette; h->rt.daylight = t->daylight; h->rt.colx = t->colx;

@@ -57,18 +57,21 @@ def lib(max_obj_tiles=None):
     L.hs_semantic.argtypes = [vp, vp]
     L.hs_noise3.restype = ctypes.c_double
     L.hs_noise3.argtypes = [vp, ctypes.c_double, ctypes.c_double, ctypes.c_double]
+    L.hs_last_error.restype = ctypes.c_char_p
     _libs[key] = L
   return _libs[key]
 
 
-def simt_lib():
-  """tests/simt: the product's kernels (csrc/cr_kernels.h) on a SIMT emulator, same C interface."""
-  if 'simt' not in _libs:
+def simt_lib(max_obj_tiles=None):
+  """tests/simt: the product's kernels (csrc/cr_kernels.h) on a SIMT emulator, same C interface.
+  max_obj_tiles: build variant with a tiny object-tile cache, as lib()."""
+  key = ('simt', max_obj_tiles)
+  if key not in _libs:
     src = HERE / 'simt' / 'simt_env.cpp'
-    out = HERE / 'simt' / '_build' / 'libsimt.so'
+    out = HERE / 'simt' / '_build' / ('libsimt.so' if max_obj_tiles is None else f'libsimt_t{max_obj_tiles}.so')
     deps = [src, HERE / 'simt' / 'simt.h'] + list((HERE.parent / 'crafter_b200' / 'csrc').glob('*.h')) + [
         HERE.parent / 'include' / 'crafter_b200.h']
-    _compile(out, src, deps)
+    _compile(out, src, deps, [] if max_obj_tiles is None else [f'-DCR_MAX_OBJ_TILES={max_obj_tiles}'])
     L = ctypes.CDLL(str(out))
     vp = ctypes.c_void_p
     L.hs_create.argtypes = [ctypes.POINTER(_cabi.CrConfig), ctypes.POINTER(_cabi.CrTables),
@@ -80,8 +83,36 @@ def simt_lib():
     L.hs_semantic.argtypes = [vp, vp]
     L.hs_simt_blocks.restype = ctypes.c_long
     L.hs_frame_order.argtypes = [vp, vp, vp]
-    _libs['simt'] = L
-  return _libs['simt']
+    L.hs_last_error.restype = ctypes.c_char_p
+    L.hs_geom.argtypes = [ctypes.POINTER(_cabi.CrConfig), vp]
+    L.hs_geom_fields.restype = ctypes.c_char_p
+    _libs[key] = L
+  return _libs[key]
+
+
+def config(num_envs=1, area=(64, 64), view=(9, 9), size=(64, 64), length=10000, reward=True, auto_reset=False,
+           slot_capacity=None, n_daylight=None, seed=0, env_offset=0, item_size=(1, 1), digit_size=(1, 1)):
+  """A cr_config (include/crafter_b200.h) as Env builds it, without the render tables: enough for the
+  checks cr_create makes before it touches a buffer."""
+  return _cabi.CrConfig(
+      num_envs=num_envs, area_w=area[0], area_h=area[1], view_w=view[0], view_h=view[1], size_w=size[0],
+      size_h=size[1], length=length, reward=int(reward), auto_reset=int(auto_reset),
+      slot_capacity=slot_capacity or state_lib.default_slot_capacity(area),
+      n_daylight=n_daylight or length + 1026, item_w=item_size[0], item_h=item_size[1], digit_w=digit_size[0],
+      digit_h=digit_size[1], seed=seed, env_offset=env_offset)
+
+
+def geom(area=(64, 64), view=(9, 9), size=(64, 64)):
+  """{field: value} of what cr_create makes of a geometry (tests/simt hs_geom: the Geom fields the kernels
+  branch on and the launch decisions at the H100's shared-memory limit); ValueError with the message
+  cr_create fails with."""
+  L = simt_lib()
+  names = L.hs_geom_fields().decode().split(',')
+  out = np.zeros(len(names), np.int64)
+  cfg = config(area=area, view=view, size=size)
+  if L.hs_geom(ctypes.byref(cfg), out.ctypes.data) != 0:
+    raise ValueError(L.hs_last_error().decode())
+  return dict(zip(names, (int(v) for v in out)))
 
 
 class HostSimEnv:
@@ -183,5 +214,4 @@ class SimtEnv(HostSimEnv):
 
   @staticmethod
   def _load(max_obj_tiles):
-    assert max_obj_tiles is None
-    return simt_lib()
+    return simt_lib(max_obj_tiles)

@@ -7,6 +7,20 @@ import numpy as np
 from oracle import canon
 
 
+POISON = 0xA5  # output buffers are filled with it before a step: a frame never drawn shows it
+
+
+def frame_problem(got, want):
+  """First difference of two frames (H, W, 3), or None."""
+  bad = got != want
+  if not bad.any():
+    return None
+  y, x, c = np.argwhere(bad)[0]
+  poisoned = bool((got == POISON).all())
+  return (f'{int(bad.any(-1).sum())} pixels differ{" (frame never drawn: still poisoned)" if poisoned else ""}, '
+          f'first at (y={y}, x={x}): {got[y, x].tolist()} vs oracle {want[y, x].tolist()}')
+
+
 def to_numpy(x):
   return x.detach().cpu().numpy() if hasattr(x, 'detach') else np.asarray(x)
 

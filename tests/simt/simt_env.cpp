@@ -70,14 +70,61 @@ void install(Handle *h) {
   LAUNCH2(k_install, h->is_default, grid, INSTALL_THREADS, 0, h->g, h->st);
 }
 
+const char *g_error = "";
+
+// The launch decisions of create_on_device (crafter_kernels.cu) for a geometry; nullptr or the message
+// cr_create fails with.  `final_obs`: the caller wants terminal frames.
+const char *plan(Handle *h, bool final_obs) {
+  Geom &g = h->g;
+  auto on = [](const char *name) { const char *v = getenv(name); return v && v[0] == '1'; };
+  h->is_default = geom_is_default(g) && !on("CRAFTER_B200_NO_SPECIALIZE");
+  h->update_smem = UPDATE_WPB * update_smem_per_warp(g);
+  if (h->update_smem > MAX_SMEM) return "view too large for the update window";
+  h->balance_smem = balance_smem(g);
+  h->balance_threads = g.NCH * 3 > 4 * BALANCE_THREADS ? BALANCE_THREADS_MAX : BALANCE_THREADS;
+  if (h->balance_smem > MAX_SMEM) return "area too large for k_balance";
+  const size_t tile = align16((size_t)g.sw * g.sh * 3);
+  if (g.tile_cache && render_tile_offset(g) > MAX_SMEM) g.tile_cache = 0;
+  const size_t fixed = render_tile_offset(g);
+  if (fixed > MAX_SMEM) return "unit too large for the tile cache";
+  h->render_staged = fixed + tile <= MAX_SMEM / 2;
+  h->render_smem = fixed + (h->render_staged ? tile : 0);
+  if (!h->render_staged) h->is_default = 0;
+  h->terminal_smem = terminal_smem(g, h->render_smem);
+  if (final_obs && (!h->render_staged || !g.tile_cache || h->terminal_smem > MAX_SMEM))
+    return "final_obs needs a frame that fits the shared-memory staging";
+  return nullptr;
+}
+
 }  // namespace
 
 extern "C" {
 
+const char *hs_last_error() { return g_error; }
+
+// What cr_create would make of a configuration: the Geom fields the kernels branch on and the launch
+// decisions, in the order of hs_geom_fields().  Returns 0, or -2 with hs_last_error() set.
+const char *hs_geom_fields() {
+  return "sw,sh,vw,vh,ux,uy,bx,by,gy,item_rows,g4_log2,band_rows,tile_cache,NCH,render_staged,is_default,"
+         "balance_threads,terminal_ok";
+}
+int hs_geom(const cr_config *c, int64_t *out) {
+  Handle h = Handle();
+  const Geom &g = h.g;
+  const char *msg = geom_from_config(*c, h.g);
+  if (!msg) msg = plan(&h, false);
+  if (msg) { g_error = msg; return -2; }
+  const int terminal_ok = plan(&h, true) == nullptr;
+  const int64_t v[] = {g.sw, g.sh, g.vw, g.vh, g.ux, g.uy, g.bx, g.by, g.gy, g.item_rows, g.g4_log2, g.band_rows,
+                       g.tile_cache, g.NCH, h.render_staged, h.is_default, h.balance_threads, terminal_ok};
+  memcpy(out, v, sizeof(v));
+  return 0;
+}
+
 int hs_create(const cr_config *c, const cr_tables *t, const cr_state *s, Handle **out) {
   Handle *h = new Handle();
   Geom &g = h->g;
-  if (geom_from_config(*c, g)) { delete h; return -2; }
+  if (const char *msg = geom_from_config(*c, g)) { g_error = msg; delete h; return -2; }
   state_from_abi(*s, h->st);
   {  // library-owned in crafter_kernels.cu: frame order, the tick's frame flags, the views k_view prepares
     const size_t head = align16((size_t)c->num_envs * (sizeof(int32_t) + 1));
@@ -92,21 +139,10 @@ int hs_create(const cr_config *c, const cr_tables *t, const cr_state *s, Handle 
   h->rt.vignette = t->vignette; h->rt.daylight = t->daylight; h->rt.colx = t->colx;
   h->rt.rowy = t->rowy;
   h->auto_reset = c->auto_reset;
-  auto on = [](const char *name) { const char *v = getenv(name); return v && v[0] == '1'; };
   auto off = [](const char *name) { const char *v = getenv(name); return v && v[0] == '0'; };
-  h->is_default = geom_is_default(g) && !on("CRAFTER_B200_NO_SPECIALIZE");
   g.draw_prefetch = !off("CRAFTER_B200_DRAW_PREFETCH");
   g.incr_census = !off("CRAFTER_B200_INCR_CENSUS") && h->st.chunk_cnt != nullptr;
-  h->update_smem = UPDATE_WPB * update_smem_per_warp(g);
-  h->balance_smem = balance_smem(g);
-  h->balance_threads = g.NCH * 3 > 4 * BALANCE_THREADS ? BALANCE_THREADS_MAX : BALANCE_THREADS;
-  const size_t tile = align16((size_t)g.sw * g.sh * 3);
-  const size_t fixed = render_tile_offset(g);
-  h->render_staged = fixed + tile <= MAX_SMEM / 2;
-  h->render_smem = fixed + (h->render_staged ? tile : 0);
-  if (!h->render_staged) h->is_default = 0;
-  h->terminal_smem = terminal_smem(g, h->render_smem);
-  if (h->st.final_obs && (!h->render_staged || !g.tile_cache || h->terminal_smem > MAX_SMEM)) { delete h; return -3; }
+  if (const char *msg = plan(h, h->st.final_obs != nullptr)) { g_error = msg; free(h->st.frame_order); delete h; return -3; }
   *out = h;
   return 0;
 }

@@ -34,12 +34,12 @@ from crafter_b200 import rules
 from crafter_b200 import state as state_lib
 from oracle import canon
 from oracle import oracle_env
+from tests.parity import POISON, frame_problem
 
 pytestmark = pytest.mark.gpu
 
 STEPS = 1300
 SAMPLE = 512
-POISON = 0xA5
 HOST_STEPS = range(1001, 1101)  # step numbers run through Env.step_host (default config)
 SEED = 0
 
@@ -69,17 +69,6 @@ def gpu_player(env):
 def gpu_canonical(env, i, arrays):
   return state_lib.canonical(*(arrays[k][i] for k in ('mat', 'ents', 'inventory', 'achievements', 'pstate',
                                                        'touched')), env._area)
-
-
-def frame_problem(got, want):
-  """First difference of two frames, or None."""
-  bad = got != want
-  if not bad.any():
-    return None
-  y, x, c = np.argwhere(bad)[0]
-  poisoned = bool((got == POISON).all())
-  return (f'{int(bad.any(-1).sum())} pixels differ{" (frame never drawn: still poisoned)" if poisoned else ""}, '
-          f'first at (y={y}, x={x}): {got[y, x].tolist()} vs oracle {want[y, x].tolist()}')
 
 
 def check_rows(where, name, got, want, env_ids=None, fields=None):

@@ -6,41 +6,102 @@ generated last), explicit reset(mask) between auto-resets, the terminal frame of
 import numpy as np
 import pytest
 
+from crafter_b200 import rules
+from crafter_b200 import state as state_lib
 from oracle import canon
 from tests import hostsim_env
 from tests import parity
 from tests.golden_util import Fixture
 
 
-def check_against_oracle(make_env, to_numpy, length, steps, K=3, seed=40, **kwargs):
+SLEEP = rules.ACTIONS.index('sleep')
+SLEEPING = len(rules.ITEMS) + len(rules.ACHIEVEMENTS) + 4  # in the canonical player vector (oracle/canon.py)
+
+
+def _put(array, col, values):
+  """array[:, col] = values for a state array of either kind (numpy on the CPU envs, torch on the GPU)."""
+  values = np.asarray(values)
+  if not isinstance(array, np.ndarray):
+    import torch
+    values = torch.as_tensor(values, dtype=array.dtype, device=array.device)
+  array[:, col] = values
+
+
+def same_frame(where, got, want):
+  problem = parity.frame_problem(got, want)
+  assert problem is None, where + (problem,)
+
+
+def check_against_oracle(make_env, to_numpy, length, steps, K=3, seed=40, start_steps=None, boost=None,
+                         sleep_bias=0.0, final_obs=False, action_seed=3, env_offset=0, **kwargs):
   """auto_reset=True against the C oracle with reset-on-done: after a finished episode the batch
-  shows the first frame / state of the next one (DESIGN.md 'Semantics added by batching')."""
+  shows the first frame / state of the next one (DESIGN.md 'Semantics added by batching').
+  Env i is the oracle's Env(seed=seed + env_offset + i).  Every step: reward, done, canonical state and
+  obs.  With final_obs, also the terminal frame and semantic map the reference returns with done=True
+  (env.py:96,118), drawn after the step's balance (env.py:90-95), which only this frame can tell.  At
+  the end: info['semantic'].
+
+  Right after reset(), both sides can be moved to where short runs reach the branches of interest:
+  start_steps   the step counter of each env (the oracle through an export / import round trip), so
+                that nightfall (step 148) and the length limit fall inside the run
+  boost         {item: count per env}, e.g. the 'unknown' digit of counts of 10 or more, or low energy
+                so that sleep takes effect
+  sleep_bias    the share of actions replaced by 'sleep'
+
+  Returns what the run reached: episodes, terminal_frames, night_frames, sleeping_night_frames."""
   from oracle import oracle_env
-  env = make_env(num_envs=K, seed=seed, length=length, auto_reset=True, **kwargs)
-  refs = [oracle_env.OracleEnv(seed=seed + i, length=length, **kwargs) for i in range(K)]
+  env = make_env(num_envs=K, seed=seed, length=length, auto_reset=True, env_offset=env_offset,
+                 **(dict(final_obs=True) if final_obs else {}), **kwargs)
+  refs = [oracle_env.OracleEnv(seed=seed + env_offset + i, length=length, **kwargs) for i in range(K)]
   obs = to_numpy(env.reset())
   for i, ref in enumerate(refs):
-    assert (ref.reset() == obs[i]).all(), ('reset', i)
-  rs = np.random.RandomState(3)
-  episodes = 0
+    same_frame(('reset', i), obs[i], ref.reset())
+  for item, counts in (boost or {}).items():
+    _put(env.state['inventory'], rules.ITEMS.index(item), counts)
+    for i, ref in enumerate(refs):
+      ref.set_inventory({item: int(counts[i])})
+  if start_steps is not None:
+    _put(env.state['pstate'], state_lib.PS['step'], np.asarray(start_steps, np.int32))
+    for i, ref in enumerate(refs):
+      ref.import_state(ref.export_state(), int(start_steps[i]), 1, oracle_env.world_seed(seed + env_offset + i, 1))
+  rs = np.random.RandomState(action_seed)
+  reached = dict(episodes=0, terminal_frames=0, night_frames=0, sleeping_night_frames=0)
   for t in range(steps):
     actions = rs.randint(0, 17, K).astype(np.int32)
-    obs, reward, done = env.step(actions)[:3]
-    obs, reward, done = to_numpy(obs), to_numpy(reward), to_numpy(done).astype(bool)
+    if sleep_bias:
+      actions[rs.rand(K) < sleep_bias] = SLEEP
+    out = env.step(actions)
+    obs, reward, done = to_numpy(out[0]), to_numpy(out[1]), to_numpy(out[2]).astype(bool)
+    if final_obs:
+      final = to_numpy(env.final_obs if hasattr(env, 'final_obs') else out[3]['final_observation'])
+      final_sem = to_numpy(env.final_semantic if hasattr(env, 'final_semantic') else out[3]['final_semantic'])
     for i, ref in enumerate(refs):
+      where = (length, t, i)
       o, r, d = ref.step(int(actions[i]))
-      assert np.float32(r) == reward[i] and d == bool(done[i]), (length, t, i)
+      assert np.float32(r) == reward[i] and d == bool(done[i]), where
       if d:
+        if final_obs:
+          same_frame(where + ('terminal frame',), final[i], o)
+          assert (ref.semantic() == final_sem[i]).all(), where + ('terminal semantic',)
+          reached['terminal_frames'] += 1
         o = ref.reset()
-        episodes += 1
-      assert canon.diff(ref.export_state(), env.snapshot(i)) is None, (length, t, i)
-      assert (o == obs[i]).all(), (length, t, i, 'obs')
-  return episodes
+        reached['episodes'] += 1
+      st = ref.export_state()
+      problem = canon.diff(st, env.snapshot(i))
+      assert problem is None, where + (problem,)
+      same_frame(where + ('obs',), obs[i], o)
+      if st['daylight'] < 0.5:
+        reached['night_frames'] += 1
+        reached['sleeping_night_frames'] += int(st['player'][SLEEPING] != 0)
+  semantic = to_numpy(env.semantic())
+  for i, ref in enumerate(refs):
+    assert (ref.semantic() == semantic[i]).all(), ('semantic', i)
+  return reached
 
 
 @pytest.mark.parametrize('length', [1, 2, 3, 7])
 def test_back_to_back_resets(length):
-  episodes = check_against_oracle(hostsim_env.HostSimEnv, np.asarray, length, steps=14)
+  episodes = check_against_oracle(hostsim_env.HostSimEnv, np.asarray, length, steps=14)['episodes']
   assert episodes >= 3 * (14 // length)
 
 
@@ -79,32 +140,9 @@ def test_mixed_resets_and_masks():
 def check_terminal_frames(make_env, to_numpy, length, steps, K=3, seed=11, **kwargs):
   """auto_reset=True, final_obs=True: when an episode ends inside step(), obs shows the first frame of
   the next episode and info['final_observation'] / the env's final_obs buffer the frame the reference
-  returns with done=True (env.py:96,118) -- drawn after the step's balance (env.py:90-95), which only
-  this frame can tell.  Also the terminal inventory / achievements (env.py:108-115)."""
-  from oracle import oracle_env
-  env = make_env(num_envs=K, seed=seed, length=length, auto_reset=True, final_obs=True, **kwargs)
-  refs = [oracle_env.OracleEnv(seed=seed + i, length=length, **kwargs) for i in range(K)]
-  obs = to_numpy(env.reset())
-  for i, ref in enumerate(refs):
-    assert (ref.reset() == obs[i]).all()
-  rs = np.random.RandomState(8)
-  ended = 0
-  for t in range(steps):
-    actions = rs.randint(0, 17, K).astype(np.int32)
-    out = env.step(actions)
-    obs, done = to_numpy(out[0]), to_numpy(out[2]).astype(bool)
-    final = to_numpy(env.final_obs if hasattr(env, 'final_obs') else out[3]['final_observation'])
-    final_sem = to_numpy(env.final_semantic if hasattr(env, 'final_semantic') else out[3]['final_semantic'])
-    for i, ref in enumerate(refs):
-      o, r, d = ref.step(int(actions[i]))
-      assert d == bool(done[i]), (t, i)
-      if d:
-        assert (o == final[i]).all(), (length, t, i, 'terminal frame')
-        assert (ref.semantic() == final_sem[i]).all(), (length, t, i, 'terminal semantic')
-        ended += 1
-        o = ref.reset()
-      assert (o == obs[i]).all(), (length, t, i, 'obs')
-  return ended
+  returns with done=True.  Returns the number of terminal frames compared."""
+  return check_against_oracle(make_env, to_numpy, length, steps, K, seed, final_obs=True, action_seed=8,
+                              **kwargs)['terminal_frames']
 
 
 @pytest.mark.parametrize('length', [1, 10, 20])
