@@ -250,7 +250,8 @@ struct State {
   // incremental census (null: every balance tick re-counts): grass, path cells of every chunk, kept current by wr_mat
   int32_t *chunk_cnt;      // [B][NCH][2]
   uint8_t *final_obs;      // [B][sh][sw][3] or null: the terminal frame of an env that was regenerated inside the step
-  uint8_t *final_semantic; // [B][NC] or null (needs final_obs): its terminal info['semantic']
+  uint8_t *final_semantic; // [B][NC] or null (needs final_obs or final_local): its terminal info['semantic']
+  uint8_t *final_local;    // [B][gx][gy] or null: the terminal local semantic window (cr_step_local)
 };
 
 CR_DEV uint8_t *next_mat_of(const State &st, const Geom &g, int env) { return st.next_mat + (size_t)env * g.NC; }

@@ -503,6 +503,54 @@ __host__ __device__ inline size_t terminal_smem(const Geom &g, size_t render_sme
   return need > render_smem ? need : render_smem;
 }
 
+// ---- the local semantic window (cr_step_local, cr_local): the cells LocalView draws (engine.py:165-176),
+// each as its info['semantic'] id (semantic_cell), 0 outside the map; [gx][gy] bytes, x-major.  `lane` of
+// `nlanes` threads stride over the cells: consecutive threads write consecutive bytes.
+__device__ __forceinline__ void local_window(const Geom &g, const State &st, int env, int lane, int nlanes,
+                                             uint8_t *out) {
+  const int32_t *ps = st.pstate + (size_t)env * PS_COUNT;
+  const int x0 = ps[PS_PX] - g.gx / 2, y0 = ps[PS_PY] - g.gy / 2;  // engine.py:161
+  const int cells = g.gx * g.gy;
+  for (int c = lane; c < cells; c += nlanes) {
+    const int i = c / g.gy, j = c - i * g.gy;
+    const int wx = x0 + i, wy = y0 + j;
+    uint8_t v = 0;
+    if (wx >= 0 && wx < g.W && wy >= 0 && wy < g.H) v = semantic_cell(g, st, env, wx * g.H + wy);
+    out[c] = v;
+  }
+}
+
+// ---- k_local: the window of every env, one warp per env (replaces the frame kernel in cr_step_local) --
+constexpr int LOCAL_WPB = 4;
+template <bool DEF>
+__global__ void __launch_bounds__(LOCAL_WPB * 32) k_local(Geom g, State st, uint8_t *__restrict__ out) {
+  geom_specialize<DEF>(g);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int env = blockIdx.x * LOCAL_WPB + warp;
+  if (env >= g.B) return;
+  local_window(g, st, env, lane, 32, out + (size_t)env * g.gx * g.gy);
+}
+
+// ---- k_final_local (final_local): k_terminal without the frame.  The terminal window of every env about
+// to be regenerated, after the step's balance when it is due (env.py:90-95), one CTA of balance_threads per
+// listed env, before k_install_map; the terminal info['semantic'] too when final_semantic is set.
+template <bool DEF>
+__global__ void __launch_bounds__(BALANCE_THREADS_MAX) k_final_local(Geom g, State st, const double *__restrict__ daylight) {
+  geom_specialize<DEF>(g);
+  CR_DYN_SMEM(smem);
+  const int nthreads = DEF ? BALANCE_THREADS : (int)blockDim.x;
+  const int count = *st.reset_count;
+  for (int r = blockIdx.x; r < count; r += gridDim.x) {
+    const int env = st.reset_list[r];
+    if (st.pstate[(size_t)env * PS_COUNT + PS_STEP] % 10 == 0) balance_env(g, st, daylight, env, threadIdx.x, nthreads, smem);
+    __syncthreads();
+    local_window(g, st, env, threadIdx.x, nthreads, st.final_local + (size_t)env * g.gx * g.gy);
+    if (st.final_semantic)
+      for (int c = threadIdx.x; c < g.NC; c += nthreads) st.final_semantic[(size_t)env * g.NC + c] = semantic_cell(g, st, env, c);
+    __syncthreads();
+  }
+}
+
 // cr_error_flags: OR of the envs' sticky error bits
 __global__ void k_error_or(Geom g, State st, int32_t *out) {
   int v = 0;

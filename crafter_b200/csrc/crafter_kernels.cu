@@ -10,7 +10,11 @@
 //                                                    +-> k_seed (ahead) -------------------------+
 //
 // The work lists' counters are cleared behind their last readers, on the side streams.  k_terminal only
-// runs when the caller asked for the terminal frames (final_obs).  Measured and NOT kept
+// runs when the caller asked for the terminal frames (final_obs).
+//
+// cr_step_local (no frame; the local semantic window instead) captures the same graph with three changes: no
+// k_view, k_post without its frame-order CTA, and k_local in place of k_render; k_final_local takes
+// k_terminal's place when the caller asked for terminal windows (final_local).  Measured and NOT kept
 // (DESIGN.md 4.2): drawing the envs the tick left final beside k_post (predicates,
 // compact lists, a launch of their own), a one-launch tick, a work queue between the tick and the frames
 // with programmatic dependent launch, persistent frame CTAs, world generation moved beside the next tick,
@@ -118,7 +122,7 @@ struct cr_handle {
   cudaEvent_t t_ev[TK_COUNT][2];
   double t_ms[TK_COUNT];
   int64_t t_n;
-  GraphSlot slots[2];  // cached step graphs: [0] device buffers only, [1] with the host copies
+  GraphSlot slots[3];  // cached step graphs: [0] device buffers only, [1] with the host copies, [2] cr_step_local
   // cr_step_host: D2H of reward/done inside the graph
   float *d2h_reward;
   uint8_t *d2h_done;
@@ -206,6 +210,14 @@ int launch_render(cr_handle *h, uint8_t *obs, cudaStream_t s, const int32_t *env
   CR_CUDA(cudaGetLastError());
   return 1;
 }
+// the local semantic window of every env (k_local) into out[B][gx][gy]
+int launch_local(cr_handle *h, uint8_t *out, cudaStream_t s) {
+  tmark(h, TK_RENDER, 0, s);
+  CR_LAUNCH(k_local, h->is_default, (h->g.B + LOCAL_WPB - 1) / LOCAL_WPB, LOCAL_WPB * 32, 0, s, h->g, h->st, out);
+  tmark(h, TK_RENDER, 1, s);
+  CR_CUDA(cudaGetLastError());
+  return 1;
+}
 // render on `s`, worldgen prefetch for the reset list on the side stream, joined back into `s`.
 int launch_render_and_prefetch(cr_handle *h, uint8_t *obs, cudaStream_t s, int seeded) {
   CR_CUDA(cudaEventRecord(h->ev_fork, s));
@@ -229,9 +241,10 @@ int enqueue_d2h(cr_handle *h, const float *reward, const uint8_t *done, cudaStre
   return 0;
 }
 
-// Enqueue one tick; returns the number of kernels or a negative error.
+// Enqueue one tick; returns the number of kernels or a negative error.  With `local` (cr_step_local) the
+// step ends in the local semantic windows instead of the frames (see the graph at the top).
 int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, uint8_t *done,
-                 cudaStream_t s) {
+                 cudaStream_t s, uint8_t *local = nullptr) {
   const Geom &g = h->g;
   const State &st = h->st;
   int n = 0, k;
@@ -255,7 +268,7 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
     if ((k = enqueue_d2h(h, reward, done, h->side2)) < 0) return k;
     CR_CUDA(cudaEventRecord(h->ev_d2h, h->side2));
   }
-  if (st.frame_view) {  // views + tile plans of the envs the tick left final, beside k_post
+  if (st.frame_view && !local) {  // views + tile plans of the envs the tick left final, beside k_post
     CR_CUDA(cudaStreamWaitEvent(h->side3, h->ev_fork, 0));
     CR_LAUNCH(k_view, h->is_default, (g.B + VIEW_WPB - 1) / VIEW_WPB, VIEW_WPB * 32, 0, h->side3, g, st, h->rt);
     CR_CUDA(cudaGetLastError());
@@ -268,7 +281,15 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
     //   side   [k_terminal] -> k_install_map -> k_install -> (k_wg_mat -> k_wg_obj || k_seed ahead) --^
     // The render needs both the balanced and the re-installed envs; world generation only the install.
     CR_CUDA(cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-    if (st.final_obs) {
+    if (local) {
+      if (st.final_local) {
+        const int grid = g.B < h->num_sms * 2 ? g.B : h->num_sms * 2;
+        CR_LAUNCH(k_final_local, h->is_default, grid, h->balance_threads, h->balance_smem, h->side, g, st,
+                  h->rt.daylight);
+        CR_CUDA(cudaGetLastError());
+        n += 1;
+      }
+    } else if (st.final_obs) {
       const int grid = g.B < h->num_sms * 2 ? g.B : h->num_sms * 2;
       CR_LAUNCH(k_terminal, h->is_default, grid, RENDER_THREADS, h->terminal_smem, h->side, g, st, h->rt);
       CR_CUDA(cudaGetLastError());
@@ -284,9 +305,10 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
   }
   const int bal_ctas = g.B < h->num_sms * 4 ? g.B : h->num_sms * 4;
   tmark(h, TK_BALANCE, 0, s);
-  // one more CTA than the balance needs: it orders the step's frames, night frames first (frame_partition)
-  CR_LAUNCH(k_post, h->is_default, bal_ctas + (st.frame_order ? 1 : 0), h->balance_threads, h->balance_smem, s, g, st,
-            h->rt.daylight, bal_ctas);
+  // one more CTA than the balance needs in a frame step: it orders the step's frames, night frames first
+  // (frame_partition)
+  CR_LAUNCH(k_post, h->is_default, bal_ctas + (st.frame_order && !local ? 1 : 0), h->balance_threads, h->balance_smem,
+            s, g, st, h->rt.daylight, bal_ctas);
   tmark(h, TK_BALANCE, 1, s);
   CR_CUDA(cudaGetLastError());
   n += 1;
@@ -295,8 +317,9 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
   CR_CUDA(cudaMemsetAsync(st.balance_count, 0, sizeof(int32_t), h->side2));
   CR_CUDA(cudaEventRecord(h->ev_bal, h->side2));
   if (h->auto_reset) CR_CUDA(cudaStreamWaitEvent(s, h->ev_inst, 0));
-  if (st.frame_view) CR_CUDA(cudaStreamWaitEvent(s, h->ev_view, 0));
-  if ((k = launch_render(h, obs, s, st.frame_order, -1, 1, st.frame_view != nullptr)) < 0) return k;
+  if (st.frame_view && !local) CR_CUDA(cudaStreamWaitEvent(s, h->ev_view, 0));
+  if ((k = local ? launch_local(h, local, s) : launch_render(h, obs, s, st.frame_order, -1, 1, st.frame_view != nullptr)) < 0)
+    return k;
   n += k;
   CR_CUDA(cudaStreamWaitEvent(s, h->ev_bal, 0));
   if (h->auto_reset) CR_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
@@ -306,7 +329,7 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
 
 void destroy_handle(cr_handle *h) {
   if (!h) return;
-  for (int i = 0; i < 2; ++i)
+  for (int i = 0; i < 3; ++i)
     if (h->slots[i].exec) cudaGraphExecDestroy(h->slots[i].exec);
   cudaStream_t streams[] = {h->side, h->side2, h->side3};
   for (cudaStream_t st : streams)
@@ -372,6 +395,10 @@ int create_on_device(cr_handle *h, const cr_config *c, const cr_tables *t, const
   if (h->balance_smem > (size_t)max_smem) return fail_msg("area too large for k_balance");
   CR_CUDA(raise_smem((const void *)k_post<true>, h->balance_smem));
   CR_CUDA(raise_smem((const void *)k_post<false>, h->balance_smem));
+  if (h->st.final_local) {  // terminal windows: the balance scratch only
+    CR_CUDA(raise_smem((const void *)k_final_local<true>, h->balance_smem));
+    CR_CUDA(raise_smem((const void *)k_final_local<false>, h->balance_smem));
+  }
   const size_t tile = align16((size_t)g.sw * g.sh * 3);
   // a tile cache that does not fit beside the frame's tables (a unit of 32 x 32 texels: 54 tiles of 4 KB,
   // e.g. render(512) at view 16) is dropped: every cell per pixel
@@ -403,6 +430,40 @@ int create_on_device(cr_handle *h, const cr_config *c, const cr_tables *t, const
   cudaEvent_t *evs[] = {&h->ev_mat, &h->ev_ahead, &h->ev_inst, &h->ev_d2h, &h->ev_fork, &h->ev_join, &h->ev_post, &h->ev_bal,
                         &h->ev_view};
   for (cudaEvent_t *e : evs) CR_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  return 0;
+}
+
+// One step through the cached graph of `gs` (captured again when a buffer changed), or eagerly.
+int run_step(cr_handle *h, GraphSlot &gs, const int32_t *actions, uint8_t *obs, float *reward, uint8_t *done,
+             uint8_t *local, cudaStream_t s) {
+  bool legacy = s == nullptr || s == cudaStreamLegacy;
+  if (!h->use_graph || legacy) {
+    int n = enqueue_step(h, actions, obs, reward, done, s, local);
+    if (n < 0) return n;
+    h->launches += n;
+    if (h->timing && h->auto_reset && tcollect(h, s)) return fail_msg("timing: stream synchronisation failed");
+    return 0;
+  }
+  const void *out = local ? (const void *)local : (const void *)obs;
+  if (!gs.exec || gs.actions != actions || gs.obs != out || gs.reward != reward || gs.done != done ||
+      gs.reward_host != h->d2h_reward || gs.done_host != h->d2h_done) {
+    if (gs.exec) { cudaGraphExecDestroy(gs.exec); gs.exec = nullptr; }
+    cudaGraph_t graph = nullptr;
+    CR_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    int n = enqueue_step(h, actions, obs, reward, done, s, local);
+    cudaError_t end = cudaStreamEndCapture(s, &graph);
+    if (n < 0) { if (graph) cudaGraphDestroy(graph); return n; }
+    if (end != cudaSuccess) return fail("cudaStreamEndCapture", end, __LINE__);
+    cudaError_t inst = cudaGraphInstantiate(&gs.exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (inst != cudaSuccess) { gs.exec = nullptr; return fail("cudaGraphInstantiate", inst, __LINE__); }
+    gs.actions = actions; gs.obs = out; gs.reward = reward; gs.done = done;
+    gs.reward_host = h->d2h_reward; gs.done_host = h->d2h_done;
+    gs.kernels = n;
+  }
+  CR_CUDA(cudaGraphLaunch(gs.exec, s));
+  h->launches += gs.kernels;
+  if (h->timing && h->auto_reset && tcollect(h, s)) return fail_msg("timing: stream synchronisation failed");
   return 0;
 }
 
@@ -475,36 +536,15 @@ int cr_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, u
             void *stream) {
   if (!h || !actions || !obs || !reward || !done) return fail_msg("null argument");
   DeviceGuard on_device(h->device);
-  cudaStream_t s = (cudaStream_t)stream;
-  bool legacy = s == nullptr || s == cudaStreamLegacy;
-  if (!h->use_graph || legacy) {
-    int n = enqueue_step(h, actions, obs, reward, done, s);
-    if (n < 0) return n;
-    h->launches += n;
-    if (h->timing && h->auto_reset && tcollect(h, s)) return fail_msg("timing: stream synchronisation failed");
-    return 0;
-  }
-  GraphSlot &gs = h->slots[h->d2h_reward ? 1 : 0];  // device-only step and host-buffer step
-  if (!gs.exec || gs.actions != actions || gs.obs != obs || gs.reward != reward || gs.done != done ||
-      gs.reward_host != h->d2h_reward || gs.done_host != h->d2h_done) {
-    if (gs.exec) { cudaGraphExecDestroy(gs.exec); gs.exec = nullptr; }
-    cudaGraph_t graph = nullptr;
-    CR_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    int n = enqueue_step(h, actions, obs, reward, done, s);
-    cudaError_t end = cudaStreamEndCapture(s, &graph);
-    if (n < 0) { if (graph) cudaGraphDestroy(graph); return n; }
-    if (end != cudaSuccess) return fail("cudaStreamEndCapture", end, __LINE__);
-    cudaError_t inst = cudaGraphInstantiate(&gs.exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (inst != cudaSuccess) { gs.exec = nullptr; return fail("cudaGraphInstantiate", inst, __LINE__); }
-    gs.actions = actions; gs.obs = obs; gs.reward = reward; gs.done = done;
-    gs.reward_host = h->d2h_reward; gs.done_host = h->d2h_done;
-    gs.kernels = n;
-  }
-  CR_CUDA(cudaGraphLaunch(gs.exec, s));
-  h->launches += gs.kernels;
-  if (h->timing && h->auto_reset && tcollect(h, s)) return fail_msg("timing: stream synchronisation failed");
-  return 0;
+  // device-only step and host-buffer step
+  return run_step(h, h->slots[h->d2h_reward ? 1 : 0], actions, obs, reward, done, nullptr, (cudaStream_t)stream);
+}
+
+int cr_step_local(cr_handle *h, const int32_t *actions, uint8_t *local_out, float *reward, uint8_t *done,
+                  void *stream) {
+  if (!h || !actions || !local_out || !reward || !done) return fail_msg("null argument");
+  DeviceGuard on_device(h->device);
+  return run_step(h, h->slots[2], actions, nullptr, reward, done, local_out, (cudaStream_t)stream);
 }
 
 int cr_step_host(cr_handle *h, const int32_t *actions_host, uint8_t *obs_host, float *reward_host,
@@ -561,6 +601,15 @@ int cr_semantic(cr_handle *h, uint8_t *out, void *stream) {
   k_semantic<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->g, h->st, out);
   CR_CUDA(cudaGetLastError());
   h->launches += 1;
+  return 0;
+}
+
+int cr_local(cr_handle *h, uint8_t *out, void *stream) {
+  if (!h || !out) return fail_msg("null argument");
+  DeviceGuard on_device(h->device);
+  int k = launch_local(h, out, (cudaStream_t)stream);
+  if (k < 0) return k;
+  h->launches += k;
   return 0;
 }
 

@@ -18,6 +18,23 @@ from . import tables as tables_lib
 
 DiscreteSpace = collections.namedtuple('DiscreteSpace', 'n')  # env.py:18-21 (gym is optional)
 BoxSpace = collections.namedtuple('BoxSpace', 'low, high, shape, dtype')
+OBSERVATIONS = ('rgb', 'semantic')
+# player.facing as (dx, dy) by the facing index of the player record (objects.py:33-34: left, right, up, down)
+FACING = ((-1, 0), (1, 0), (0, -1), (0, 1))
+
+
+def player_facing(ents):
+  """info['facing']: the player's facing (dx, dy) as int32 (B, 2), decoded from the `aux` field (bits 48-63)
+  of the player's slot record (slot 1) in the ents tensor (B, slot_capacity) int64."""
+  table = torch.tensor(FACING, dtype=torch.int32, device=ents.device)
+  return table[(ents[:, 1] >> 48).long()]
+
+
+def daylight_at(pstate, daylight):
+  """info['daylight']: the daylight each env's last step used (env.py:135-139), float32 (B,): the daylight
+  table at the env's step counter, clamped to the table's end as the kernels clamp it."""
+  step = pstate[:, state_lib.PS['step']].long().clamp(0, daylight.numel() - 1)
+  return daylight[step].float()
 
 
 class Info(dict):
@@ -25,7 +42,12 @@ class Info(dict):
   first access: 'semantic' (engine.py:251-264), 'discount' (env.py:111) and -- for auto_reset, where
   'inventory' / 'achievements' of an env that just finished already belong to its next episode --
   'final_inventory' / 'final_achievements' / 'final_player_pos' / 'final_observation' / 'final_semantic': the terminal transition as the
-  reference's info shows it (rows of envs with done=False hold their last terminal values or zeros)."""
+  reference's info shows it (rows of envs with done=False hold their last terminal values or zeros).
+
+  What the frame shows beyond the semantic ids (a semantic window shows every player as id 13):
+  'facing' int32 (B, 2), the player's facing (dx, dy); 'sleeping' bool (B,); 'daylight' float32 (B,), the
+  daylight of the step.  'local_semantic': the local semantic window (see Env.local_semantic), which is
+  `obs` itself with observation='semantic'."""
 
   def __init__(self, env, *args, **kwargs):
     super().__init__(*args, **kwargs)
@@ -47,9 +69,18 @@ class Info(dict):
     elif key == 'final_player_pos':
       value = env._state['final_stats'][:, 40:42]
     elif key in ('final_observation', 'final_semantic'):
-      if env._final_obs is None:
+      if env._final_semantic is None:
         raise KeyError(f"{key} needs Env(..., auto_reset=True, final_obs=True)")
-      value = env._final_obs if key == 'final_observation' else env._final_semantic.view(env.num_envs, *env._area)
+      final = env._final_local if env._observation == 'semantic' else env._final_obs
+      value = final if key == 'final_observation' else env._final_semantic.view(env.num_envs, *env._area)
+    elif key == 'facing':
+      value = player_facing(env._state['ents'])
+    elif key == 'sleeping':
+      value = env._state['pstate'][:, state_lib.PS['sleeping']] != 0
+    elif key == 'daylight':
+      value = daylight_at(env._state['pstate'], env._daylight)
+    elif key == 'local_semantic':
+      value = env._local if env._observation == 'semantic' else env.local_semantic()
     else:
       raise KeyError(key)
     self[key] = value
@@ -68,6 +99,13 @@ class Env:
                 env i plays the reference's `Env(seed=seed + env_offset + i)`
   final_obs     with auto_reset: also draw the frame of the step that ended an episode (the one the
                 reference returns with done=True, env.py:96,118) into info['final_observation']
+  observation   'rgb' (the reference's frames) or 'semantic': no frame is drawn inside the step, and obs is
+                the local semantic window, uint8 (num_envs, gx, gy) with gx = view[0] and gy = view[1] minus
+                the item rows, x-major like info['semantic']: the id of each cell the frame's local view
+                shows (LocalView, engine.py:155-180; ids of SemanticView, engine.py:251-264: materials
+                1..12, objects 13..18), 0 outside the map.  render() and info['semantic'] still work on
+                demand; with final_obs, info['final_observation'] is the terminal window.  step_host is
+                not available.
 
   Randomness is counter-based (Philox keyed by the per-episode world seed, see DESIGN.md), so a
   batch is reproducible and independent of how it is sharded.  Returned tensors are views of the
@@ -76,7 +114,7 @@ class Env:
 
   def __init__(self, num_envs=1, area=(64, 64), view=(9, 9), size=(64, 64), reward=True,
                length=10000, seed=None, device=None, auto_reset=False, env_offset=0,
-               slot_capacity=None, final_obs=False):
+               slot_capacity=None, final_obs=False, observation='rgb'):
     if not torch.cuda.is_available():
       raise RuntimeError('crafter_b200 needs a CUDA device (sm_90a); there is no CPU fallback')
     self._lib = _cabi.load()
@@ -100,6 +138,10 @@ class Env:
     if final_obs and not auto_reset:
       raise ValueError('final_obs only makes sense with auto_reset=True (otherwise obs IS the terminal frame)')
     self._want_final_obs = bool(final_obs)
+    if observation not in OBSERVATIONS:
+      raise ValueError(f"observation must be one of {OBSERVATIONS}, not {observation!r}")
+    self._observation = observation
+    self._grid = tuple(int(v) for v in geo['grid'])  # the local view (env.py:42-44): the window's shape
     self._env_offset = int(env_offset)
     self._capacity = int(slot_capacity or state_lib.default_slot_capacity(self._area))
     # env.py:106: length None / 0 = no time limit.  Daylight (env.py:135-139) is a host-built table, so an
@@ -118,8 +160,9 @@ class Env:
     self._needs_reset = True
     # raw addresses of the fixed buffers: the per-step calls below hand them to the C ABI without
     # touching torch again (the library switches to its own device itself, see DeviceGuard)
-    self._ptrs = (self._actions.data_ptr(), self._obs.data_ptr(), self._reward_buf.data_ptr(),
-                  self._done.data_ptr())
+    out = self._local if observation == 'semantic' else self._obs
+    self._ptrs = (self._actions.data_ptr(), out.data_ptr(), self._reward_buf.data_ptr(), self._done.data_ptr())
+    self._step_fn = self._lib.cr_step_local if observation == 'semantic' else self._lib.cr_step
     self._stream_ptr = self._stream.cuda_stream
     self._host_key, self._host_ptrs = None, None
 
@@ -154,9 +197,13 @@ class Env:
       # grass / path cells per chunk, maintained by the terrain writes instead of being re-counted by
       # every balance tick (DESIGN.md 4.2; =0 goes back to the census for A/B runs)
       self._state['chunk_cnt'] = z(B, nch * 2, dtype=torch.int32)
-    self._obs = z(B, int(self._size[1]), int(self._size[0]), 3, dtype=torch.uint8)
-    self._final_obs = z(B, int(self._size[1]), int(self._size[0]), 3, dtype=torch.uint8) if self._want_final_obs else None
-    self._final_semantic = z(B, nc, dtype=torch.uint8) if self._want_final_obs else None
+    frames = self._observation == 'rgb'
+    self._obs = z(B, int(self._size[1]), int(self._size[0]), 3, dtype=torch.uint8) if frames else None
+    self._local = None if frames else z(B, *self._grid, dtype=torch.uint8)
+    want = self._want_final_obs
+    self._final_obs = z(B, int(self._size[1]), int(self._size[0]), 3, dtype=torch.uint8) if want and frames else None
+    self._final_local = z(B, *self._grid, dtype=torch.uint8) if want and not frames else None
+    self._final_semantic = z(B, nc, dtype=torch.uint8) if want else None
     self._reward_buf = z(B, dtype=torch.float32)
     self._zero_reward = z(B, dtype=torch.float32)  # reward=False (env.py:116-117); info['reward'] keeps the real one
     self._done = z(B, dtype=torch.bool)
@@ -177,8 +224,11 @@ class Env:
         env_offset=self._env_offset)
     tabs = _cabi.CrTables(**{k: v.data_ptr() for k, v in dev.items()})
     st = _cabi.CrState(**{k: v.data_ptr() for k, v in self._state.items()})
-    if self._final_obs is not None and size == tuple(int(v) for v in self._size):
-      st.final_obs = self._final_obs.data_ptr()
+    if self._final_semantic is not None and size == tuple(int(v) for v in self._size):
+      if self._final_obs is not None:
+        st.final_obs = self._final_obs.data_ptr()
+      else:
+        st.final_local = self._final_local.data_ptr()
       st.final_semantic = self._final_semantic.data_ptr()
     handle = ctypes.c_void_p()
     _cabi.check(self._lib.cr_create(
@@ -209,7 +259,14 @@ class Env:
     return self._device
 
   @property
+  def observation(self):
+    """'rgb' or 'semantic' (see the class docstring)."""
+    return self._observation
+
+  @property
   def observation_space(self):
+    if self._observation == 'semantic':
+      return BoxSpace(0, 18, self._grid, np.uint8)
     return BoxSpace(0, 255, (int(self._size[1]), int(self._size[0]), 3), np.uint8)
 
   @property
@@ -240,10 +297,14 @@ class Env:
           raise RuntimeError('the first reset() must cover every env (envs outside the mask have no world yet)')
         ptr = mask.data_ptr()
       s = self._enter()
-      _cabi.check(self._lib.cr_reset(self._handle, ptr, self._obs.data_ptr(), s))
+      if self._observation == 'semantic':  # no frame: the windows of the state the reset left
+        _cabi.check(self._lib.cr_reset(self._handle, ptr, None, s))
+        _cabi.check(self._lib.cr_local(self._handle, self._local.data_ptr(), s))
+      else:
+        _cabi.check(self._lib.cr_reset(self._handle, ptr, self._obs.data_ptr(), s))
       self._exit()
     self._needs_reset = False
-    return self._obs
+    return self._local if self._observation == 'semantic' else self._obs
 
   # ---- Env.step (env.py:83-118) ---------------------------------------------------------------
   def step(self, actions):
@@ -254,12 +315,13 @@ class Env:
       a = torch.as_tensor(actions)
       self._actions.copy_(a.reshape(self._num_envs), non_blocking=True)
     s = self._enter()
-    _cabi.check(self._lib.cr_step(self._handle, *self._ptrs, s))
+    _cabi.check(self._step_fn(self._handle, *self._ptrs, s))
     self._exit()
     info = Info(
         self, inventory=self._state['inventory'], achievements=self._state['achievements'],
         player_pos=self._state['pstate'][:, 12:14], reward=self._reward_buf)
-    return self._obs, self._reward_buf if self._reward else self._zero_reward, self._done, info
+    obs = self._local if self._observation == 'semantic' else self._obs
+    return obs, self._reward_buf if self._reward else self._zero_reward, self._done, info
 
   @property
   def actions_buffer(self):
@@ -269,6 +331,8 @@ class Env:
   def step_host(self, actions_pinned, reward_pinned, done_pinned, obs_pinned=None):
     """One tick through `cr_step_host`: pinned host buffers in and out, copies and the stream
     synchronisation included -- the path a non-torch caller of the reference's step() binds."""
+    if self._observation != 'rgb':
+      raise RuntimeError("step_host draws frames: it is not available with observation='semantic'")
     if self._needs_reset:
       raise RuntimeError('call reset() before step()')
     key = (id(actions_pinned), id(reward_pinned), id(done_pinned), id(obs_pinned))
@@ -311,6 +375,16 @@ class Env:
       out = torch.empty(self._num_envs, *self._area, dtype=torch.uint8, device=self._device)
       s = self._enter()
       _cabi.check(self._lib.cr_semantic(self._handle, out.data_ptr(), s))
+      self._exit()
+    return out
+
+  def local_semantic(self):
+    """The local semantic window of every env as the state stands: (num_envs, gx, gy) uint8, the obs of
+    observation='semantic' (see the class docstring).  Reads only the cells around each player."""
+    with torch.cuda.device(self._device):
+      out = torch.empty(self._num_envs, *self._grid, dtype=torch.uint8, device=self._device)
+      s = self._enter()
+      _cabi.check(self._lib.cr_local(self._handle, out.data_ptr(), s))
       self._exit()
     return out
 

@@ -19,7 +19,7 @@
 extern "C" {
 #endif
 
-#define CR_ABI_VERSION 3
+#define CR_ABI_VERSION 4
 
 typedef struct cr_handle cr_handle;
 
@@ -78,7 +78,11 @@ typedef struct cr_state {
    * reference returns with done=True (env.py:96,118), for the envs regenerated inside cr_step;
    * rows of other envs are left alone.  [B][size_h][size_w][3] */
   uint8_t *final_obs;
-  uint8_t *final_semantic; /* optional with final_obs: the terminal info['semantic'] of those envs, [B][W][H] */
+  uint8_t *final_semantic; /* optional with final_obs or final_local: the terminal info['semantic'] of those envs, [B][W][H] */
+  /* Optional (NULL: off), auto_reset only: the local semantic window (see cr_local) of the step that ended an
+   * episode, for the envs regenerated inside cr_step_local, taken after the step's balance; rows of other envs
+   * are left alone.  [B][view_w][view_h - item rows].  cr_step writes final_obs, cr_step_local this. */
+  uint8_t *final_local;
 } cr_state;
 
 int cr_abi_version(void);
@@ -91,13 +95,22 @@ int cr_create(const cr_config *cfg, const cr_tables *tables, const cr_state *sta
 int cr_destroy(cr_handle *h);
 
 /* Env.reset (env.py:70-81) for the envs whose mask byte is non-zero (mask == NULL: all).
- * Writes the first observation of the reset envs into obs[B][size_h][size_w][3]. */
+ * Writes the first observation of the reset envs into obs[B][size_h][size_w][3] (obs == NULL: no frame is
+ * drawn; cr_local then gives the first local semantic windows). */
 int cr_reset(cr_handle *h, const uint8_t *mask, uint8_t *obs, void *stream);
 
 /* Env.step (env.py:83-118): actions int32[B] in, obs / reward float32[B] / done uint8[B] out.
  * The per-env info tensors are the cr_state buffers themselves (zero copy). */
 int cr_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, uint8_t *done,
             void *stream);
+
+/* The same tick without a frame: the local semantic window of every env into local_out[B][gx][gy] uint8
+ * instead of obs, where gx = view_w and gy = view_h - item rows (env.py:42-44), x-major like cr_semantic.
+ * Cell (x, y) holds the info['semantic'] id (SemanticView, engine.py:251-264) of map cell
+ * player.pos + (x, y) - (gx / 2, gy / 2), the cells LocalView draws (engine.py:165-176), and 0 outside
+ * the map.  One handle serves both kinds of step; each keeps its own cached graph. */
+int cr_step_local(cr_handle *h, const int32_t *actions, uint8_t *local_out, float *reward, uint8_t *done,
+                  void *stream);
 
 /* Same tick with HOST buffers: copies actions in and reward/done (and obs when non-NULL) out and
  * synchronises the stream -- what a non-torch caller of the reference's step() would bind. */
@@ -116,6 +129,10 @@ int cr_render_envs(cr_handle *h, const int32_t *env_ids, int n, uint8_t *obs, vo
 /* SemanticView (engine.py:251-264): out[B][W][H] uint8, info['semantic']. */
 int cr_semantic(cr_handle *h, uint8_t *out, void *stream);
 
+/* The local semantic window of every env as the state stands (the window cr_step_local returns):
+ * out[B][gx][gy] uint8.  After cr_reset(h, mask, NULL, s) it gives the first window of the reset envs. */
+int cr_local(cr_handle *h, uint8_t *out, void *stream);
+
 /* After the caller has written `mat` itself (state restore, tests): recount what the library keeps
  * incrementally about the terrain (the per-chunk counts of chunk_cnt; a no-op without that buffer
  * or with CRAFTER_B200_INCR_CENSUS=0). */
@@ -132,7 +149,8 @@ int64_t cr_launch_count(const cr_handle *h);
 /* Profiling aid: with CRAFTER_B200_TIMING=1 in the environment the step runs eagerly with events
  * around every kernel, with =2 it stays one graph and the events are nodes of it; writes the mean
  * device ms of [update, install, render, seed, wg_mat, wg_obj,
- * seed_ahead, balance] since the last call and returns the number of steps averaged (0 = off). */
+ * seed_ahead, balance] since the last call and returns the number of steps averaged (0 = off).
+ * In a cr_step_local step the `render` entry times the window kernel (k_local) that replaces the frames. */
 int64_t cr_timing(cr_handle *h, double *out_ms);
 
 #ifdef __cplusplus
