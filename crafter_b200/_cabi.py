@@ -7,7 +7,7 @@ import pathlib
 
 ROOT = pathlib.Path(__file__).resolve().parent
 LIB_PATH = pathlib.Path(os.environ.get('CRAFTER_B200_LIB', ROOT / '_lib' / 'libcrafter_b200.so'))  # override: A/B builds
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 
 class CrConfig(ctypes.Structure):
@@ -36,12 +36,15 @@ class CrState(ctypes.Structure):
       # optional terminal frames of auto-reset (NULL: off)
       'final_obs', 'final_semantic',
       # optional terminal local semantic windows of auto-reset (NULL: off)
-      'final_local')]
+      'final_local',
+      # optional terminal symbolic vectors of auto-reset (NULL: off)
+      'final_symbolic')]
 
 
 EXPORTS = ('cr_abi_version', 'cr_last_error', 'cr_create', 'cr_destroy', 'cr_reset', 'cr_step',
            'cr_step_host', 'cr_render', 'cr_render_envs', 'cr_semantic', 'cr_recount', 'cr_launch_count',
-           'cr_timing', 'cr_source_hash', 'cr_error_flags', 'cr_step_local', 'cr_local')
+           'cr_timing', 'cr_source_hash', 'cr_error_flags', 'cr_step_local', 'cr_local',
+           'cr_step_symbolic', 'cr_symbolic')
 
 _lib = None
 
@@ -58,11 +61,13 @@ def declare(lib, prefix='cr_'):
     lib.cr_reset.argtypes = [vp, vp, vp, vp]
     lib.cr_step.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.cr_step_local.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.cr_step_symbolic.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.cr_step_host.argtypes = [vp] * 10
     lib.cr_render.argtypes = [vp, vp, vp]
     lib.cr_render_envs.argtypes = [vp, vp, ctypes.c_int, vp, vp]
     lib.cr_semantic.argtypes = [vp, vp, vp]
     lib.cr_local.argtypes = [vp, vp, vp]
+    lib.cr_symbolic.argtypes = [vp, vp, vp]
     lib.cr_recount.argtypes = [vp, vp]
     lib.cr_launch_count.argtypes = [vp]
     lib.cr_launch_count.restype = ctypes.c_int64

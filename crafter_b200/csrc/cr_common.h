@@ -252,6 +252,7 @@ struct State {
   uint8_t *final_obs;      // [B][sh][sw][3] or null: the terminal frame of an env that was regenerated inside the step
   uint8_t *final_semantic; // [B][NC] or null (needs final_obs or final_local): its terminal info['semantic']
   uint8_t *final_local;    // [B][gx][gy] or null: the terminal local semantic window (cr_step_local)
+  float *final_symbolic;   // [B][22 gx gy + 22] or null: the terminal symbolic vector (cr_step_symbolic)
 };
 
 CR_DEV uint8_t *next_mat_of(const State &st, const Geom &g, int env) { return st.next_mat + (size_t)env * g.NC; }

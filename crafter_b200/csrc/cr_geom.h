@@ -78,6 +78,7 @@ inline void state_from_abi(const cr_state &s, State &st) {
   st.frame_order = nullptr; st.frame_night = nullptr; st.frame_view = nullptr;  // library-owned (cr_create)
   st.chunk_cnt = s.chunk_cnt;
   st.final_obs = s.final_obs; st.final_semantic = s.final_semantic; st.final_local = s.final_local;
+  st.final_symbolic = s.final_symbolic;
 }
 
 }  // namespace cr

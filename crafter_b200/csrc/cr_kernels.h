@@ -531,9 +531,72 @@ __global__ void __launch_bounds__(LOCAL_WPB * 32) k_local(Geom g, State st, uint
   local_window(g, st, env, lane, 32, out + (size_t)env * g.gx * g.gy);
 }
 
-// ---- k_final_local (final_local): k_terminal without the frame.  The terminal window of every env about
-// to be regenerated, after the step's balance when it is due (env.py:90-95), one CTA of balance_threads per
-// listed env, before k_install_map; the terminal info['semantic'] too when final_semantic is set.
+// ---- the symbolic observation (cr_step_symbolic, cr_symbolic): D = 22 gx gy + 22 float32 per env, laid out
+// as include/crafter_b200.h describes.  Two phases with the group's threads synchronised between them:
+// symbolic_codes puts the window's cell codes (symbolic_cell, 0 outside the map) into `codes`, gx * gy bytes
+// of shared memory; symbolic_write then writes the vector, `lane` of `nlanes` threads striding over it, so
+// consecutive threads write consecutive floats and every byte of the row is written once.
+constexpr int SYM_CELL_CH = 22;  // per window cell: materials 1..12, then the 10 object channels
+constexpr int SYM_TAIL = N_ITEMS + 4 + 1 + 1;  // inventory, facing, sleeping, daylight
+constexpr int SYM_MAX_CELLS = 256;  // the largest window geom_from_config accepts
+__host__ __device__ inline int symbolic_dim(const Geom &g) { return SYM_CELL_CH * g.gx * g.gy + SYM_TAIL; }
+
+__device__ __forceinline__ void symbolic_codes(const Geom &g, const State &st, int env, int lane, int nlanes,
+                                               uint8_t *codes) {
+  const int32_t *ps = st.pstate + (size_t)env * PS_COUNT;
+  const int x0 = ps[PS_PX] - g.gx / 2, y0 = ps[PS_PY] - g.gy / 2;  // engine.py:161, as local_window
+  const int cells = g.gx * g.gy;
+  for (int c = lane; c < cells; c += nlanes) {
+    const int i = c / g.gy, j = c - i * g.gy;
+    const int wx = x0 + i, wy = y0 + j;
+    uint8_t v = 0;
+    if (wx >= 0 && wx < g.W && wy >= 0 && wy < g.H) v = symbolic_cell(g, st, env, wx * g.H + wy);
+    codes[c] = v;
+  }
+}
+
+__device__ __forceinline__ void symbolic_write(const Geom &g, const State &st, const double *__restrict__ daylight,
+                                               int env, int lane, int nlanes, const uint8_t *codes, float *out) {
+  const int32_t *ps = st.pstate + (size_t)env * PS_COUNT;
+  const int32_t *inv = st.inventory + (size_t)env * N_ITEMS;
+  const int map = SYM_CELL_CH * g.gx * g.gy;
+  for (int i = lane; i < map + SYM_TAIL; i += nlanes) {
+    float v;
+    if (i < map) {
+      const int c = i / SYM_CELL_CH, ch = i - c * SYM_CELL_CH;
+      const int code = codes[c];
+      v = ch < 12 ? (code & 15) == ch + 1 : (code >> 4) == ch - 11;
+    } else {
+      const int t = i - map;
+      if (t < N_ITEMS) v = (float)inv[t] / 9.0f;  // IEEE division: numpy's float32(k) / float32(9)
+      else if (t < N_ITEMS + 4) v = st.ents[(size_t)env * g.CAP + 1].aux == t - N_ITEMS;  // the player's facing
+      else if (t == N_ITEMS + 4) v = ps[PS_SLEEPING] != 0;
+      else v = (float)daylight[imin(ps[PS_STEP], g.n_daylight - 1)];  // info['daylight']
+    }
+    out[i] = v;
+  }
+}
+
+// ---- k_symbolic: the vector of every env, one warp per env (replaces the frame kernel in cr_step_symbolic) -
+template <bool DEF>
+__global__ void __launch_bounds__(LOCAL_WPB * 32)
+k_symbolic(Geom g, State st, const double *__restrict__ daylight, float *__restrict__ out) {
+  geom_specialize<DEF>(g);
+  __shared__ uint8_t s_codes[LOCAL_WPB][SYM_MAX_CELLS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int env = blockIdx.x * LOCAL_WPB + warp;
+  if (env >= g.B) return;
+  symbolic_codes(g, st, env, lane, 32, s_codes[warp]);
+  __syncwarp();
+  symbolic_write(g, st, daylight, env, lane, 32, s_codes[warp], out + (size_t)env * symbolic_dim(g));
+}
+
+// ---- k_final_local (final_local, final_symbolic): k_terminal without the frame.  The terminal window or
+// terminal symbolic vector of every env about to be regenerated, after the step's balance when it is due
+// (env.py:90-95), one CTA of balance_threads per listed env, before k_install_map; the terminal
+// info['semantic'] too when final_semantic is set.  The launch passes the one of final_local / final_symbolic
+// that belongs to its kind of step; the vector's cell codes reuse the balance scratch once the balance is done.
+static_assert(sizeof(PlayerS) >= SYM_MAX_CELLS, "the balance scratch holds a window's symbolic cell codes");
 template <bool DEF>
 __global__ void __launch_bounds__(BALANCE_THREADS_MAX) k_final_local(Geom g, State st, const double *__restrict__ daylight) {
   geom_specialize<DEF>(g);
@@ -544,7 +607,14 @@ __global__ void __launch_bounds__(BALANCE_THREADS_MAX) k_final_local(Geom g, Sta
     const int env = st.reset_list[r];
     if (st.pstate[(size_t)env * PS_COUNT + PS_STEP] % 10 == 0) balance_env(g, st, daylight, env, threadIdx.x, nthreads, smem);
     __syncthreads();
-    local_window(g, st, env, threadIdx.x, nthreads, st.final_local + (size_t)env * g.gx * g.gy);
+    if (st.final_local) local_window(g, st, env, threadIdx.x, nthreads, st.final_local + (size_t)env * g.gx * g.gy);
+    if (st.final_symbolic) {
+      uint8_t *codes = reinterpret_cast<uint8_t *>(smem);
+      symbolic_codes(g, st, env, threadIdx.x, nthreads, codes);
+      __syncthreads();
+      symbolic_write(g, st, daylight, env, threadIdx.x, nthreads, codes,
+                     st.final_symbolic + (size_t)env * symbolic_dim(g));
+    }
     if (st.final_semantic)
       for (int c = threadIdx.x; c < g.NC; c += nthreads) st.final_semantic[(size_t)env * g.NC + c] = semantic_cell(g, st, env, c);
     __syncthreads();

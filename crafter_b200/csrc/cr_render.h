@@ -606,4 +606,19 @@ CR_DEV uint8_t semantic_cell(const Geom &g, const State &st, int env, int cell) 
   return st.mat[(size_t)env * g.NC + cell] & 0x7F;
 }
 
+// The symbolic observation's code of a map cell (cr_step_symbolic): bits 0-3 the material id 1..12, also under
+// an object; bits 4-7 one plus the object's channel 0..9 (player, cow, zombie, skeleton, arrow left / right / up
+// / down, plant, ripe plant), 0 without one.  The arrow's channel is its facing, ripe is grown > 300
+// (objects.py:361-367,402-403): what the sprite (sprite_of) shows beyond the semantic id.
+CR_DEV uint8_t symbolic_cell(const Geom &g, const State &st, int env, int cell) {
+  const int slot = st.objmap[(size_t)env * g.NC + cell];
+  int code = st.mat[(size_t)env * g.NC + cell] & 0x7F;
+  if (slot) {
+    const Ent e = st.ents[(size_t)env * g.CAP + slot];
+    const int ch = e.type == T_ARROW ? 4 + e.aux : e.type == T_PLANT ? (e.aux > 300 ? 9 : 8) : e.type - 1;
+    code |= (1 + ch) << 4;
+  }
+  return (uint8_t)code;
+}
+
 }  // namespace cr

@@ -14,7 +14,9 @@
 //
 // cr_step_local (no frame; the local semantic window instead) captures the same graph with three changes: no
 // k_view, k_post without its frame-order CTA, and k_local in place of k_render; k_final_local takes
-// k_terminal's place when the caller asked for terminal windows (final_local).  Measured and NOT kept
+// k_terminal's place when the caller asked for terminal windows (final_local).  cr_step_symbolic (the symbolic
+// vector instead) is the same graph with k_symbolic in place of k_local; its k_final_local writes the terminal
+// vectors (final_symbolic).  Measured and NOT kept
 // (DESIGN.md 4.2): drawing the envs the tick left final beside k_post (predicates,
 // compact lists, a launch of their own), a one-launch tick, a work queue between the tick and the frames
 // with programmatic dependent launch, persistent frame CTAs, world generation moved beside the next tick,
@@ -122,7 +124,8 @@ struct cr_handle {
   cudaEvent_t t_ev[TK_COUNT][2];
   double t_ms[TK_COUNT];
   int64_t t_n;
-  GraphSlot slots[3];  // cached step graphs: [0] device buffers only, [1] with the host copies, [2] cr_step_local
+  GraphSlot slots[4];  // cached step graphs: [0] device buffers only, [1] with the host copies, [2] cr_step_local,
+                       // [3] cr_step_symbolic
   // cr_step_host: D2H of reward/done inside the graph
   float *d2h_reward;
   uint8_t *d2h_done;
@@ -218,6 +221,15 @@ int launch_local(cr_handle *h, uint8_t *out, cudaStream_t s) {
   CR_CUDA(cudaGetLastError());
   return 1;
 }
+// the symbolic vector of every env (k_symbolic) into out[B][D]
+int launch_symbolic(cr_handle *h, float *out, cudaStream_t s) {
+  tmark(h, TK_RENDER, 0, s);
+  CR_LAUNCH(k_symbolic, h->is_default, (h->g.B + LOCAL_WPB - 1) / LOCAL_WPB, LOCAL_WPB * 32, 0, s, h->g, h->st,
+            h->rt.daylight, out);
+  tmark(h, TK_RENDER, 1, s);
+  CR_CUDA(cudaGetLastError());
+  return 1;
+}
 // render on `s`, worldgen prefetch for the reset list on the side stream, joined back into `s`.
 int launch_render_and_prefetch(cr_handle *h, uint8_t *obs, cudaStream_t s, int seeded) {
   CR_CUDA(cudaEventRecord(h->ev_fork, s));
@@ -242,11 +254,13 @@ int enqueue_d2h(cr_handle *h, const float *reward, const uint8_t *done, cudaStre
 }
 
 // Enqueue one tick; returns the number of kernels or a negative error.  With `local` (cr_step_local) the
-// step ends in the local semantic windows instead of the frames (see the graph at the top).
+// step ends in the local semantic windows instead of the frames, with `symbolic` (cr_step_symbolic) in the
+// symbolic vectors (see the graph at the top).
 int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, uint8_t *done,
-                 cudaStream_t s, uint8_t *local = nullptr) {
+                 cudaStream_t s, uint8_t *local = nullptr, float *symbolic = nullptr) {
   const Geom &g = h->g;
   const State &st = h->st;
+  const bool frameless = local || symbolic;
   int n = 0, k;
   // The work lists' counters are zero whenever a step begins: each is cleared behind its last reader
   // (k_post; the world-generation branch) on a side stream, off the critical path -- the memset node in
@@ -268,7 +282,7 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
     if ((k = enqueue_d2h(h, reward, done, h->side2)) < 0) return k;
     CR_CUDA(cudaEventRecord(h->ev_d2h, h->side2));
   }
-  if (st.frame_view && !local) {  // views + tile plans of the envs the tick left final, beside k_post
+  if (st.frame_view && !frameless) {  // views + tile plans of the envs the tick left final, beside k_post
     CR_CUDA(cudaStreamWaitEvent(h->side3, h->ev_fork, 0));
     CR_LAUNCH(k_view, h->is_default, (g.B + VIEW_WPB - 1) / VIEW_WPB, VIEW_WPB * 32, 0, h->side3, g, st, h->rt);
     CR_CUDA(cudaGetLastError());
@@ -281,10 +295,14 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
     //   side   [k_terminal] -> k_install_map -> k_install -> (k_wg_mat -> k_wg_obj || k_seed ahead) --^
     // The render needs both the balanced and the re-installed envs; world generation only the install.
     CR_CUDA(cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-    if (local) {
-      if (st.final_local) {
+    if (frameless) {
+      // the terminal output of this kind of step only: k_final_local writes what its State points to
+      State fst = st;
+      if (symbolic) fst.final_local = nullptr;
+      else fst.final_symbolic = nullptr;
+      if (fst.final_local || fst.final_symbolic) {
         const int grid = g.B < h->num_sms * 2 ? g.B : h->num_sms * 2;
-        CR_LAUNCH(k_final_local, h->is_default, grid, h->balance_threads, h->balance_smem, h->side, g, st,
+        CR_LAUNCH(k_final_local, h->is_default, grid, h->balance_threads, h->balance_smem, h->side, g, fst,
                   h->rt.daylight);
         CR_CUDA(cudaGetLastError());
         n += 1;
@@ -307,7 +325,7 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
   tmark(h, TK_BALANCE, 0, s);
   // one more CTA than the balance needs in a frame step: it orders the step's frames, night frames first
   // (frame_partition)
-  CR_LAUNCH(k_post, h->is_default, bal_ctas + (st.frame_order && !local ? 1 : 0), h->balance_threads, h->balance_smem,
+  CR_LAUNCH(k_post, h->is_default, bal_ctas + (st.frame_order && !frameless ? 1 : 0), h->balance_threads, h->balance_smem,
             s, g, st, h->rt.daylight, bal_ctas);
   tmark(h, TK_BALANCE, 1, s);
   CR_CUDA(cudaGetLastError());
@@ -317,8 +335,10 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
   CR_CUDA(cudaMemsetAsync(st.balance_count, 0, sizeof(int32_t), h->side2));
   CR_CUDA(cudaEventRecord(h->ev_bal, h->side2));
   if (h->auto_reset) CR_CUDA(cudaStreamWaitEvent(s, h->ev_inst, 0));
-  if (st.frame_view && !local) CR_CUDA(cudaStreamWaitEvent(s, h->ev_view, 0));
-  if ((k = local ? launch_local(h, local, s) : launch_render(h, obs, s, st.frame_order, -1, 1, st.frame_view != nullptr)) < 0)
+  if (st.frame_view && !frameless) CR_CUDA(cudaStreamWaitEvent(s, h->ev_view, 0));
+  if ((k = local      ? launch_local(h, local, s)
+           : symbolic ? launch_symbolic(h, symbolic, s)
+                      : launch_render(h, obs, s, st.frame_order, -1, 1, st.frame_view != nullptr)) < 0)
     return k;
   n += k;
   CR_CUDA(cudaStreamWaitEvent(s, h->ev_bal, 0));
@@ -329,7 +349,7 @@ int enqueue_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *rewa
 
 void destroy_handle(cr_handle *h) {
   if (!h) return;
-  for (int i = 0; i < 3; ++i)
+  for (int i = 0; i < 4; ++i)
     if (h->slots[i].exec) cudaGraphExecDestroy(h->slots[i].exec);
   cudaStream_t streams[] = {h->side, h->side2, h->side3};
   for (cudaStream_t st : streams)
@@ -395,7 +415,7 @@ int create_on_device(cr_handle *h, const cr_config *c, const cr_tables *t, const
   if (h->balance_smem > (size_t)max_smem) return fail_msg("area too large for k_balance");
   CR_CUDA(raise_smem((const void *)k_post<true>, h->balance_smem));
   CR_CUDA(raise_smem((const void *)k_post<false>, h->balance_smem));
-  if (h->st.final_local) {  // terminal windows: the balance scratch only
+  if (h->st.final_local || h->st.final_symbolic) {  // terminal windows / vectors: the balance scratch only
     CR_CUDA(raise_smem((const void *)k_final_local<true>, h->balance_smem));
     CR_CUDA(raise_smem((const void *)k_final_local<false>, h->balance_smem));
   }
@@ -435,22 +455,22 @@ int create_on_device(cr_handle *h, const cr_config *c, const cr_tables *t, const
 
 // One step through the cached graph of `gs` (captured again when a buffer changed), or eagerly.
 int run_step(cr_handle *h, GraphSlot &gs, const int32_t *actions, uint8_t *obs, float *reward, uint8_t *done,
-             uint8_t *local, cudaStream_t s) {
+             uint8_t *local, float *symbolic, cudaStream_t s) {
   bool legacy = s == nullptr || s == cudaStreamLegacy;
   if (!h->use_graph || legacy) {
-    int n = enqueue_step(h, actions, obs, reward, done, s, local);
+    int n = enqueue_step(h, actions, obs, reward, done, s, local, symbolic);
     if (n < 0) return n;
     h->launches += n;
     if (h->timing && h->auto_reset && tcollect(h, s)) return fail_msg("timing: stream synchronisation failed");
     return 0;
   }
-  const void *out = local ? (const void *)local : (const void *)obs;
+  const void *out = local ? (const void *)local : symbolic ? (const void *)symbolic : (const void *)obs;
   if (!gs.exec || gs.actions != actions || gs.obs != out || gs.reward != reward || gs.done != done ||
       gs.reward_host != h->d2h_reward || gs.done_host != h->d2h_done) {
     if (gs.exec) { cudaGraphExecDestroy(gs.exec); gs.exec = nullptr; }
     cudaGraph_t graph = nullptr;
     CR_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    int n = enqueue_step(h, actions, obs, reward, done, s, local);
+    int n = enqueue_step(h, actions, obs, reward, done, s, local, symbolic);
     cudaError_t end = cudaStreamEndCapture(s, &graph);
     if (n < 0) { if (graph) cudaGraphDestroy(graph); return n; }
     if (end != cudaSuccess) return fail("cudaStreamEndCapture", end, __LINE__);
@@ -537,14 +557,22 @@ int cr_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, u
   if (!h || !actions || !obs || !reward || !done) return fail_msg("null argument");
   DeviceGuard on_device(h->device);
   // device-only step and host-buffer step
-  return run_step(h, h->slots[h->d2h_reward ? 1 : 0], actions, obs, reward, done, nullptr, (cudaStream_t)stream);
+  return run_step(h, h->slots[h->d2h_reward ? 1 : 0], actions, obs, reward, done, nullptr, nullptr,
+                  (cudaStream_t)stream);
 }
 
 int cr_step_local(cr_handle *h, const int32_t *actions, uint8_t *local_out, float *reward, uint8_t *done,
                   void *stream) {
   if (!h || !actions || !local_out || !reward || !done) return fail_msg("null argument");
   DeviceGuard on_device(h->device);
-  return run_step(h, h->slots[2], actions, nullptr, reward, done, local_out, (cudaStream_t)stream);
+  return run_step(h, h->slots[2], actions, nullptr, reward, done, local_out, nullptr, (cudaStream_t)stream);
+}
+
+int cr_step_symbolic(cr_handle *h, const int32_t *actions, float *out, float *reward, uint8_t *done,
+                     void *stream) {
+  if (!h || !actions || !out || !reward || !done) return fail_msg("null argument");
+  DeviceGuard on_device(h->device);
+  return run_step(h, h->slots[3], actions, nullptr, reward, done, nullptr, out, (cudaStream_t)stream);
 }
 
 int cr_step_host(cr_handle *h, const int32_t *actions_host, uint8_t *obs_host, float *reward_host,
@@ -608,6 +636,15 @@ int cr_local(cr_handle *h, uint8_t *out, void *stream) {
   if (!h || !out) return fail_msg("null argument");
   DeviceGuard on_device(h->device);
   int k = launch_local(h, out, (cudaStream_t)stream);
+  if (k < 0) return k;
+  h->launches += k;
+  return 0;
+}
+
+int cr_symbolic(cr_handle *h, float *out, void *stream) {
+  if (!h || !out) return fail_msg("null argument");
+  DeviceGuard on_device(h->device);
+  int k = launch_symbolic(h, out, (cudaStream_t)stream);
   if (k < 0) return k;
   h->launches += k;
   return 0;

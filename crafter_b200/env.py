@@ -18,9 +18,26 @@ from . import tables as tables_lib
 
 DiscreteSpace = collections.namedtuple('DiscreteSpace', 'n')  # env.py:18-21 (gym is optional)
 BoxSpace = collections.namedtuple('BoxSpace', 'low, high, shape, dtype')
-OBSERVATIONS = ('rgb', 'semantic')
+OBSERVATIONS = ('rgb', 'semantic', 'symbolic')
 # player.facing as (dx, dy) by the facing index of the player record (objects.py:33-34: left, right, up, down)
 FACING = ((-1, 0), (1, 0), (0, -1), (0, 1))
+# The 22 channels of every window cell of observation='symbolic' (layout: include/crafter_b200.h,
+# cr_step_symbolic): one-hot of the material, set under objects too, then one-hot of the object's texture
+SYMBOLIC_CHANNELS = tuple(rules.MATERIALS) + (
+    'player', 'cow', 'zombie', 'skeleton', 'arrow-left', 'arrow-right', 'arrow-up', 'arrow-down', 'plant',
+    'plant-ripe')
+
+
+def symbolic_layout(grid):
+  """{part: slice} of the symbolic vector of a local view `grid` = (gx, gy): 'map' (22 gx gy entries, cell
+  (x, y) at (x * gy + y) * 22, channels SYMBOLIC_CHANNELS), 'inventory' (16, count / 9 in rules.ITEMS
+  order), 'facing' (4, one-hot in FACING order), 'sleeping' (1) and 'daylight' (1)."""
+  start, out = 0, {}
+  for part, n in (('map', len(SYMBOLIC_CHANNELS) * grid[0] * grid[1]), ('inventory', len(rules.ITEMS)),
+                  ('facing', len(FACING)), ('sleeping', 1), ('daylight', 1)):
+    out[part] = slice(start, start + n)
+    start += n
+  return out
 
 
 def player_facing(ents):
@@ -71,7 +88,7 @@ class Info(dict):
     elif key in ('final_observation', 'final_semantic'):
       if env._final_semantic is None:
         raise KeyError(f"{key} needs Env(..., auto_reset=True, final_obs=True)")
-      final = env._final_local if env._observation == 'semantic' else env._final_obs
+      final = {'rgb': env._final_obs, 'semantic': env._final_local, 'symbolic': env._final_symbolic}[env._observation]
       value = final if key == 'final_observation' else env._final_semantic.view(env.num_envs, *env._area)
     elif key == 'facing':
       value = player_facing(env._state['ents'])
@@ -106,6 +123,13 @@ class Env:
                 1..12, objects 13..18), 0 outside the map.  render() and info['semantic'] still work on
                 demand; with final_obs, info['final_observation'] is the terminal window.  step_host is
                 not available.
+                Or 'symbolic': no frame either, and obs is float32 (num_envs, D), D = 22 gx gy + 22 (1408
+                at the default view): the local window one-hot by material and by object texture, the
+                inventory / 9, the facing one-hot, sleeping and the daylight.  The layout is defined in
+                include/crafter_b200.h (cr_step_symbolic); decode it through SYMBOLIC_CHANNELS and
+                Env.symbolic_layout rather than by offsets.  render(), info['semantic'] and
+                local_semantic() work on demand; with final_obs, info['final_observation'] is the terminal
+                vector.  step_host is not available.
 
   Randomness is counter-based (Philox keyed by the per-episode world seed, see DESIGN.md), so a
   batch is reproducible and independent of how it is sharded.  Returned tensors are views of the
@@ -160,9 +184,9 @@ class Env:
     self._needs_reset = True
     # raw addresses of the fixed buffers: the per-step calls below hand them to the C ABI without
     # touching torch again (the library switches to its own device itself, see DeviceGuard)
-    out = self._local if observation == 'semantic' else self._obs
-    self._ptrs = (self._actions.data_ptr(), out.data_ptr(), self._reward_buf.data_ptr(), self._done.data_ptr())
-    self._step_fn = self._lib.cr_step_local if observation == 'semantic' else self._lib.cr_step
+    self._ptrs = (self._actions.data_ptr(), self._out.data_ptr(), self._reward_buf.data_ptr(), self._done.data_ptr())
+    self._step_fn = {'rgb': self._lib.cr_step, 'semantic': self._lib.cr_step_local,
+                     'symbolic': self._lib.cr_step_symbolic}[observation]
     self._stream_ptr = self._stream.cuda_stream
     self._host_key, self._host_ptrs = None, None
 
@@ -197,12 +221,15 @@ class Env:
       # grass / path cells per chunk, maintained by the terrain writes instead of being re-counted by
       # every balance tick (DESIGN.md 4.2; =0 goes back to the census for A/B runs)
       self._state['chunk_cnt'] = z(B, nch * 2, dtype=torch.int32)
-    frames = self._observation == 'rgb'
-    self._obs = z(B, int(self._size[1]), int(self._size[0]), 3, dtype=torch.uint8) if frames else None
-    self._local = None if frames else z(B, *self._grid, dtype=torch.uint8)
-    want = self._want_final_obs
-    self._final_obs = z(B, int(self._size[1]), int(self._size[0]), 3, dtype=torch.uint8) if want and frames else None
-    self._final_local = z(B, *self._grid, dtype=torch.uint8) if want and not frames else None
+    mode, want = self._observation, self._want_final_obs
+    frame, dim = (int(self._size[1]), int(self._size[0]), 3), self.symbolic_layout['daylight'].stop
+    self._obs = z(B, *frame, dtype=torch.uint8) if mode == 'rgb' else None
+    self._local = z(B, *self._grid, dtype=torch.uint8) if mode == 'semantic' else None
+    self._sym = z(B, dim, dtype=torch.float32) if mode == 'symbolic' else None
+    self._out = {'rgb': self._obs, 'semantic': self._local, 'symbolic': self._sym}[mode]  # what step() returns
+    self._final_obs = z(B, *frame, dtype=torch.uint8) if want and mode == 'rgb' else None
+    self._final_local = z(B, *self._grid, dtype=torch.uint8) if want and mode == 'semantic' else None
+    self._final_symbolic = z(B, dim, dtype=torch.float32) if want and mode == 'symbolic' else None
     self._final_semantic = z(B, nc, dtype=torch.uint8) if want else None
     self._reward_buf = z(B, dtype=torch.float32)
     self._zero_reward = z(B, dtype=torch.float32)  # reward=False (env.py:116-117); info['reward'] keeps the real one
@@ -227,8 +254,10 @@ class Env:
     if self._final_semantic is not None and size == tuple(int(v) for v in self._size):
       if self._final_obs is not None:
         st.final_obs = self._final_obs.data_ptr()
-      else:
+      elif self._final_local is not None:
         st.final_local = self._final_local.data_ptr()
+      else:
+        st.final_symbolic = self._final_symbolic.data_ptr()
       st.final_semantic = self._final_semantic.data_ptr()
     handle = ctypes.c_void_p()
     _cabi.check(self._lib.cr_create(
@@ -260,13 +289,20 @@ class Env:
 
   @property
   def observation(self):
-    """'rgb' or 'semantic' (see the class docstring)."""
+    """'rgb', 'semantic' or 'symbolic' (see the class docstring)."""
     return self._observation
+
+  @property
+  def symbolic_layout(self):
+    """{part: slice} of the symbolic vector at this env's view (see symbolic_layout())."""
+    return symbolic_layout(self._grid)
 
   @property
   def observation_space(self):
     if self._observation == 'semantic':
       return BoxSpace(0, 18, self._grid, np.uint8)
+    if self._observation == 'symbolic':
+      return BoxSpace(0, 1, (self.symbolic_layout['daylight'].stop,), np.float32)
     return BoxSpace(0, 255, (int(self._size[1]), int(self._size[0]), 3), np.uint8)
 
   @property
@@ -300,11 +336,14 @@ class Env:
       if self._observation == 'semantic':  # no frame: the windows of the state the reset left
         _cabi.check(self._lib.cr_reset(self._handle, ptr, None, s))
         _cabi.check(self._lib.cr_local(self._handle, self._local.data_ptr(), s))
+      elif self._observation == 'symbolic':  # no frame: the vectors of the state the reset left
+        _cabi.check(self._lib.cr_reset(self._handle, ptr, None, s))
+        _cabi.check(self._lib.cr_symbolic(self._handle, self._sym.data_ptr(), s))
       else:
         _cabi.check(self._lib.cr_reset(self._handle, ptr, self._obs.data_ptr(), s))
       self._exit()
     self._needs_reset = False
-    return self._local if self._observation == 'semantic' else self._obs
+    return self._out
 
   # ---- Env.step (env.py:83-118) ---------------------------------------------------------------
   def step(self, actions):
@@ -320,8 +359,7 @@ class Env:
     info = Info(
         self, inventory=self._state['inventory'], achievements=self._state['achievements'],
         player_pos=self._state['pstate'][:, 12:14], reward=self._reward_buf)
-    obs = self._local if self._observation == 'semantic' else self._obs
-    return obs, self._reward_buf if self._reward else self._zero_reward, self._done, info
+    return self._out, self._reward_buf if self._reward else self._zero_reward, self._done, info
 
   @property
   def actions_buffer(self):
@@ -332,7 +370,7 @@ class Env:
     """One tick through `cr_step_host`: pinned host buffers in and out, copies and the stream
     synchronisation included -- the path a non-torch caller of the reference's step() binds."""
     if self._observation != 'rgb':
-      raise RuntimeError("step_host draws frames: it is not available with observation='semantic'")
+      raise RuntimeError(f'step_host draws frames: it is not available with observation={self._observation!r}')
     if self._needs_reset:
       raise RuntimeError('call reset() before step()')
     key = (id(actions_pinned), id(reward_pinned), id(done_pinned), id(obs_pinned))
@@ -385,6 +423,17 @@ class Env:
       out = torch.empty(self._num_envs, *self._grid, dtype=torch.uint8, device=self._device)
       s = self._enter()
       _cabi.check(self._lib.cr_local(self._handle, out.data_ptr(), s))
+      self._exit()
+    return out
+
+  def symbolic(self):
+    """The symbolic vector of every env as the state stands: (num_envs, D) float32, the obs of
+    observation='symbolic' (see the class docstring), in any mode."""
+    with torch.cuda.device(self._device):
+      out = torch.empty(self._num_envs, self.symbolic_layout['daylight'].stop, dtype=torch.float32,
+                        device=self._device)
+      s = self._enter()
+      _cabi.check(self._lib.cr_symbolic(self._handle, out.data_ptr(), s))
       self._exit()
     return out
 

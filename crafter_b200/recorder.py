@@ -90,8 +90,9 @@ class EpisodeRecorder:
   """
 
   def __init__(self, env, directory, env_ids=(0,)):
-    if getattr(env, 'observation', 'rgb') != 'rgb':
-      raise ValueError("EpisodeRecorder records the 'image' frames of an episode; Env(..., observation='semantic') "
+    mode = getattr(env, 'observation', 'rgb')
+    if mode != 'rgb':
+      raise ValueError(f"EpisodeRecorder records the 'image' frames of an episode; Env(..., observation={mode!r}) "
                        "draws none (use observation='rgb', or StatsRecorder / VideoRecorder)")
     self._auto = bool(getattr(env, '_auto_reset', False))
     if self._auto and getattr(env, '_final_obs', None) is None:

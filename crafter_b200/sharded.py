@@ -23,7 +23,8 @@ def shard_of(total_envs, rank, world):
 class ShardedEnv:
   """`crafter_b200.Env` over the whole job: `num_envs` is the GLOBAL batch; this process steps its
   own shard on `cuda:LOCAL_RANK`.  reset()/step() return the local shard's tensors.  Keyword arguments go to
-  the env unchanged (e.g. `observation='semantic'`: `gather` takes windows as it takes frames)."""
+  the env unchanged (e.g. `observation='semantic'` or `'symbolic'`: `gather` takes windows and float32 vectors
+  as it takes frames)."""
 
   def __init__(self, num_envs, seed=0, env_factory=None, **kwargs):
     self.rank = dist.get_rank() if dist.is_initialized() else int(os.environ.get('RANK', 0))

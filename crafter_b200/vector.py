@@ -16,7 +16,8 @@ the next episode), and the terminal transition travels in `info` under gymnasium
 `terminated` = the player died (`discount` 0 in the reference, env.py:105,111), `truncated` = the
 episode hit `length` (the registration's max_episode_steps).  Arrays are torch.cuda tensors unless
 `to_numpy=True`.  With `observation='semantic'` (see `crafter_b200.Env`) the observations, `final_obs`
-included, are the local semantic windows and the spaces say so (`Box(0, 18, (gx, gy), uint8)`).
+included, are the local semantic windows and the spaces say so (`Box(0, 18, (gx, gy), uint8)`); with
+`observation='symbolic'` they are the symbolic vectors (`Box(0, 1, (D,), float32)`).
 gym / gymnasium are optional (absent in this image): with gymnasium installed the
 class derives from `gymnasium.vector.VectorEnv` and uses its spaces; `register()` adds the two ids
 when either package is importable.
@@ -39,6 +40,8 @@ class _Box:
     self.low, self.high, self.shape, self.dtype = low, high, tuple(shape), np.dtype(dtype)
 
   def sample(self):
+    if self.dtype.kind == 'f':
+      return np.random.uniform(self.low, self.high, self.shape).astype(self.dtype)
     return np.random.randint(self.low, self.high + 1, self.shape).astype(self.dtype)
 
   def contains(self, x):
@@ -81,15 +84,15 @@ class _MultiDiscrete:
     return f'MultiDiscrete({self.nvec.tolist()[:4]}...)'
 
 
-def _spaces(num_envs, obs_shape, n_actions, high=255):
+def _spaces(num_envs, obs_shape, n_actions, high=255, dtype=np.uint8):
   if _gym is not None:
     sp = _gym.spaces
-    single_obs = sp.Box(0, high, obs_shape, np.uint8)
+    single_obs = sp.Box(0, high, obs_shape, dtype)
     single_act = sp.Discrete(n_actions)
     return (single_obs, single_act, _gym.vector.utils.batch_space(single_obs, num_envs),
             _gym.vector.utils.batch_space(single_act, num_envs))
-  return (_Box(0, high, obs_shape, np.uint8), _Discrete(n_actions),
-          _Box(0, high, (num_envs,) + tuple(obs_shape), np.uint8), _MultiDiscrete([n_actions] * num_envs))
+  return (_Box(0, high, obs_shape, dtype), _Discrete(n_actions),
+          _Box(0, high, (num_envs,) + tuple(obs_shape), dtype), _MultiDiscrete([n_actions] * num_envs))
 
 
 class VectorEnv(_Base):
@@ -107,7 +110,7 @@ class VectorEnv(_Base):
     self._final = bool(final_obs)
     (self.single_observation_space, self.single_action_space, self.observation_space,
      self.action_space) = _spaces(self.num_envs, self.env.observation_space.shape, self.env.action_space.n,
-                                  self.env.observation_space.high)
+                                  self.env.observation_space.high, self.env.observation_space.dtype)
     mode = 'same_step' if kwargs['auto_reset'] else 'disabled'
     if _gym is not None and hasattr(_gym.vector, 'AutoresetMode'):
       mode = _gym.vector.AutoresetMode(mode)

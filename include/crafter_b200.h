@@ -19,7 +19,7 @@
 extern "C" {
 #endif
 
-#define CR_ABI_VERSION 4
+#define CR_ABI_VERSION 5
 
 typedef struct cr_handle cr_handle;
 
@@ -78,11 +78,15 @@ typedef struct cr_state {
    * reference returns with done=True (env.py:96,118), for the envs regenerated inside cr_step;
    * rows of other envs are left alone.  [B][size_h][size_w][3] */
   uint8_t *final_obs;
-  uint8_t *final_semantic; /* optional with final_obs or final_local: the terminal info['semantic'] of those envs, [B][W][H] */
+  uint8_t *final_semantic; /* optional with final_obs, final_local or final_symbolic: the terminal info['semantic'] of those envs, [B][W][H] */
   /* Optional (NULL: off), auto_reset only: the local semantic window (see cr_local) of the step that ended an
    * episode, for the envs regenerated inside cr_step_local, taken after the step's balance; rows of other envs
    * are left alone.  [B][view_w][view_h - item rows].  cr_step writes final_obs, cr_step_local this. */
   uint8_t *final_local;
+  /* Optional (NULL: off), auto_reset only: the symbolic vector (see cr_step_symbolic) of the step that ended an
+   * episode, for the envs regenerated inside cr_step_symbolic, taken after the step's balance; rows of other
+   * envs are left alone.  [B][D] float32. */
+  float *final_symbolic;
 } cr_state;
 
 int cr_abi_version(void);
@@ -112,6 +116,25 @@ int cr_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, u
 int cr_step_local(cr_handle *h, const int32_t *actions, uint8_t *local_out, float *reward, uint8_t *done,
                   void *stream);
 
+/* The same tick without a frame: the symbolic observation of every env into out[B][D] float32, where
+ * D = 22 * gx * gy + 22 (gx, gy as in cr_step_local; D = 1408 at the default view).  Row layout, every entry
+ * exactly 0, 1, k / 9 or a float32 rounding of the daylight table:
+ *   [0, 22 gx gy)  the local window, cell (x, y) at (x * gy + y) * 22, covering the map cell of cr_step_local's
+ *                  cell (x, y); all 22 entries 0 outside the map, else
+ *                    channels 0..11   one-hot of the material id 1..12 (data.yaml order), under objects too,
+ *                    channels 12..21  one-hot of the object's texture, if the cell holds one: player, cow,
+ *                                     zombie, skeleton, arrow left / right / up / down (its facing), plant,
+ *                                     ripe plant (grown > 300, objects.py:402-403);
+ *   then 16        the inventory in data.yaml order, float32(count) / float32(9) (IEEE division; above 1
+ *                  for counts above 9);
+ *   then 4         the player's facing, one-hot in the order left, right, up, down (objects.py:33-34);
+ *   then 1         sleeping, 0 or 1;
+ *   then 1         the daylight (env.py:135-139): float32 of tables.daylight at the env's step counter,
+ *                  clamped to the table's end.
+ * One handle serves all three kinds of step; each keeps its own cached graph. */
+int cr_step_symbolic(cr_handle *h, const int32_t *actions, float *out, float *reward, uint8_t *done,
+                     void *stream);
+
 /* Same tick with HOST buffers: copies actions in and reward/done (and obs when non-NULL) out and
  * synchronises the stream -- what a non-torch caller of the reference's step() would bind. */
 int cr_step_host(cr_handle *h, const int32_t *actions_host, uint8_t *obs_host, float *reward_host,
@@ -133,6 +156,10 @@ int cr_semantic(cr_handle *h, uint8_t *out, void *stream);
  * out[B][gx][gy] uint8.  After cr_reset(h, mask, NULL, s) it gives the first window of the reset envs. */
 int cr_local(cr_handle *h, uint8_t *out, void *stream);
 
+/* The symbolic vector of every env as the state stands (the vector cr_step_symbolic returns): out[B][D]
+ * float32.  After cr_reset(h, mask, NULL, s) it gives the first vector of the reset envs. */
+int cr_symbolic(cr_handle *h, float *out, void *stream);
+
 /* After the caller has written `mat` itself (state restore, tests): recount what the library keeps
  * incrementally about the terrain (the per-chunk counts of chunk_cnt; a no-op without that buffer
  * or with CRAFTER_B200_INCR_CENSUS=0). */
@@ -150,7 +177,8 @@ int64_t cr_launch_count(const cr_handle *h);
  * around every kernel, with =2 it stays one graph and the events are nodes of it; writes the mean
  * device ms of [update, install, render, seed, wg_mat, wg_obj,
  * seed_ahead, balance] since the last call and returns the number of steps averaged (0 = off).
- * In a cr_step_local step the `render` entry times the window kernel (k_local) that replaces the frames. */
+ * In a cr_step_local step the `render` entry times the window kernel (k_local) that replaces the frames, in a
+ * cr_step_symbolic step the vector kernel (k_symbolic). */
 int64_t cr_timing(cr_handle *h, double *out_ms);
 
 #ifdef __cplusplus
