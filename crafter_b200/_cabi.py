@@ -7,7 +7,7 @@ import pathlib
 
 ROOT = pathlib.Path(__file__).resolve().parent
 LIB_PATH = pathlib.Path(os.environ.get('CRAFTER_B200_LIB', ROOT / '_lib' / 'libcrafter_b200.so'))  # override: A/B builds
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 
 class CrConfig(ctypes.Structure):
@@ -38,13 +38,15 @@ class CrState(ctypes.Structure):
       # optional terminal local semantic windows of auto-reset (NULL: off)
       'final_local',
       # optional terminal symbolic vectors of auto-reset (NULL: off)
-      'final_symbolic')]
+      'final_symbolic',
+      # levels (NULL: cr_set_levels fails) and the world seed of the last finished episode (NULL: off)
+      'level', 'final_world_seed')]
 
 
 EXPORTS = ('cr_abi_version', 'cr_last_error', 'cr_create', 'cr_destroy', 'cr_reset', 'cr_step',
            'cr_step_host', 'cr_render', 'cr_render_envs', 'cr_semantic', 'cr_recount', 'cr_launch_count',
            'cr_timing', 'cr_source_hash', 'cr_error_flags', 'cr_step_local', 'cr_local',
-           'cr_step_symbolic', 'cr_symbolic')
+           'cr_step_symbolic', 'cr_symbolic', 'cr_set_levels')
 
 _lib = None
 
@@ -69,6 +71,7 @@ def declare(lib, prefix='cr_'):
     lib.cr_local.argtypes = [vp, vp, vp]
     lib.cr_symbolic.argtypes = [vp, vp, vp]
     lib.cr_recount.argtypes = [vp, vp]
+    lib.cr_set_levels.argtypes = [vp, vp, vp, vp]
     lib.cr_launch_count.argtypes = [vp]
     lib.cr_launch_count.restype = ctypes.c_int64
     lib.cr_error_flags.argtypes = [vp, vp, vp]

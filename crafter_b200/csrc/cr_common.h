@@ -253,6 +253,8 @@ struct State {
   uint8_t *final_semantic; // [B][NC] or null (needs final_obs or final_local): its terminal info['semantic']
   uint8_t *final_local;    // [B][gx][gy] or null: the terminal local semantic window (cr_step_local)
   float *final_symbolic;   // [B][22 gx gy + 22] or null: the terminal symbolic vector (cr_step_symbolic)
+  int32_t *level;          // [B] or null: the world seed every new episode plays, -1 = world_seed_of (cr_set_levels)
+  int32_t *final_world_seed;  // [B] or null: the world seed of the episode that ended last
 };
 
 CR_DEV uint8_t *next_mat_of(const State &st, const Geom &g, int env) { return st.next_mat + (size_t)env * g.NC; }

@@ -79,6 +79,7 @@ inline void state_from_abi(const cr_state &s, State &st) {
   st.chunk_cnt = s.chunk_cnt;
   st.final_obs = s.final_obs; st.final_semantic = s.final_semantic; st.final_local = s.final_local;
   st.final_symbolic = s.final_symbolic;
+  st.level = s.level; st.final_world_seed = s.final_world_seed;
 }
 
 }  // namespace cr

@@ -888,6 +888,7 @@ CR_DEV int env_step(const Geom &g, const State &st, const double *daylight_table
       fs[FS_DEAD] = dead ? 1 : 0;  // terminated (health <= 0) vs truncated (length reached), env.py:105-107
       for (int i = 0; i < N_ITEMS; ++i) fs[FS_INV + i] = P->inv[i];
       fs[FS_POS] = P->ps[PS_PX]; fs[FS_POS + 1] = P->ps[PS_PY];
+      if (st.final_world_seed) st.final_world_seed[env] = P->ps[PS_WORLD_SEED];  // before k_install replaces it
       P->ps[PS_EP_LENGTH] = step;
       if (auto_reset) kind |= TICK_RESET;
     }

@@ -92,7 +92,8 @@ CR_DEV void wg_seed(const Geom &g, const State &st, int env, int lane, SeedScrat
   uint8_t *perm = wg_perm_of(st, env, episode);
   uint32_t ws = 0;
   if (lane == 0) {
-    ws = world_seed_of(g.seed + g.env_offset + env, episode);
+    const int32_t level = st.level ? st.level[env] : -1;  // cr_set_levels
+    ws = level >= 0 ? (uint32_t)level : world_seed_of(g.seed + g.env_offset + env, episode);
     nm[ahead ? NM_AHEAD_EPISODE : NM_EPISODE] = episode;
     nm[ahead ? NM_AHEAD_WORLD_SEED : NM_WORLD_SEED] = (int32_t)ws;
     if (!ahead) nm[NM_SEEDED] = 1;

@@ -552,6 +552,22 @@ int cr_reset(cr_handle *h, const uint8_t *mask, uint8_t *obs, void *stream) {
   return 0;
 }
 
+int cr_set_levels(cr_handle *h, const uint8_t *mask, const int32_t *levels, void *stream) {
+  if (!h || !levels) return fail_msg("null argument");
+  if (!h->st.level) return fail_msg("cr_set_levels: the handle has no level buffer (cr_state.level is NULL)");
+  DeviceGuard on_device(h->device);
+  cudaStream_t s = (cudaStream_t)stream;
+  k_set_levels<<<(h->g.B + 255) / 256, 256, 0, s>>>(h->g.B, h->st, mask, levels);
+  CR_CUDA(cudaGetLastError());
+  h->launches += 1;
+  // the next world (only_invalid: every listed env was invalidated) and, beside its terrain, the one after it
+  int k;
+  if ((k = launch_worldgen(h, s, h->st.reset_list, h->st.reset_count, 1, 1, 0)) < 0) return k;
+  h->launches += k;
+  CR_CUDA(cudaMemsetAsync(h->st.reset_count, 0, sizeof(int32_t), s));  // zero whenever a step begins
+  return 0;
+}
+
 int cr_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, uint8_t *done,
             void *stream) {
   if (!h || !actions || !obs || !reward || !done) return fail_msg("null argument");

@@ -19,6 +19,7 @@ from . import tables as tables_lib
 DiscreteSpace = collections.namedtuple('DiscreteSpace', 'n')  # env.py:18-21 (gym is optional)
 BoxSpace = collections.namedtuple('BoxSpace', 'low, high, shape, dtype')
 OBSERVATIONS = ('rgb', 'semantic', 'symbolic')
+MAX_LEVEL = 2 ** 31 - 2  # the largest world seed of the reference, hash(...) % (2**31 - 1) (env.py:74)
 # player.facing as (dx, dy) by the facing index of the player record (objects.py:33-34: left, right, up, down)
 FACING = ((-1, 0), (1, 0), (0, -1), (0, 1))
 # The 22 channels of every window cell of observation='symbolic' (layout: include/crafter_b200.h,
@@ -54,12 +55,43 @@ def daylight_at(pstate, daylight):
   return daylight[step].float()
 
 
+def check_levels(levels, mask, num_envs):
+  """Env.set_levels' arguments checked on the host: (levels as int64, mask as bool or None), tensors on the
+  device `levels` came on.  ValueError for a non-integer dtype, a wrong shape, or a masked entry that is
+  neither -1 nor a world seed in [0, MAX_LEVEL]; entries outside the mask are not looked at."""
+  if torch.is_tensor(levels):
+    if levels.dtype.is_floating_point or levels.dtype.is_complex or levels.dtype == torch.bool:
+      raise ValueError(f'levels must be integers, not {levels.dtype}')
+    arr = levels.to(torch.int64)
+  else:
+    a = np.asarray(levels)
+    if a.dtype.kind not in 'iu':
+      raise ValueError(f'levels must be integers, not {a.dtype}')
+    if a.dtype.kind == 'u' and a.size and int(a.max()) > MAX_LEVEL:
+      raise ValueError(f'levels must be -1 or world seeds in [0, {MAX_LEVEL}]')
+    arr = torch.from_numpy(a.astype(np.int64))
+  if tuple(arr.shape) != (num_envs,):
+    raise ValueError(f'levels must have shape ({num_envs},), not {tuple(arr.shape)}')
+  if mask is not None:
+    mask = torch.as_tensor(mask, device=arr.device).to(torch.bool)
+    if tuple(mask.shape) != (num_envs,):
+      raise ValueError(f'mask must have shape ({num_envs},), not {tuple(mask.shape)}')
+  chosen = arr if mask is None else torch.where(mask, arr, -1)  # -1 is always valid
+  lo, hi = torch.stack([chosen.min(), chosen.max()]).tolist() if num_envs else (-1, -1)  # one device read
+  if lo < -1 or hi > MAX_LEVEL:
+    raise ValueError(f'levels must be -1 or world seeds in [0, {MAX_LEVEL}]')
+  return arr, mask
+
+
 class Info(dict):
   """`info` of Env.step (env.py:108-115) as batched tensors; expensive entries are computed on
   first access: 'semantic' (engine.py:251-264), 'discount' (env.py:111) and -- for auto_reset, where
   'inventory' / 'achievements' of an env that just finished already belong to its next episode --
   'final_inventory' / 'final_achievements' / 'final_player_pos' / 'final_observation' / 'final_semantic': the terminal transition as the
   reference's info shows it (rows of envs with done=False hold their last terminal values or zeros).
+  'world_seed' int32 (B,): the world seed the current episode of each env plays; 'final_world_seed' int32 (B,):
+  the world seed of the episode that ended in this step (rows with done=False hold older values or zeros) --
+  with auto_reset, what Env.reset(levels=...) needs to replay that episode (see Env.set_levels).
 
   What the frame shows beyond the semantic ids (a semantic window shows every player as id 13):
   'facing' int32 (B, 2), the player's facing (dx, dy); 'sleeping' bool (B,); 'daylight' float32 (B,), the
@@ -96,6 +128,10 @@ class Info(dict):
       value = env._state['pstate'][:, state_lib.PS['sleeping']] != 0
     elif key == 'daylight':
       value = daylight_at(env._state['pstate'], env._daylight)
+    elif key == 'world_seed':
+      value = env._state['pstate'][:, state_lib.PS['world_seed']]
+    elif key == 'final_world_seed':
+      value = env._state['final_world_seed']
     elif key == 'local_semantic':
       value = env._local if env._observation == 'semantic' else env.local_semantic()
     else:
@@ -132,7 +168,9 @@ class Env:
                 vector.  step_host is not available.
 
   Randomness is counter-based (Philox keyed by the per-episode world seed, see DESIGN.md), so a
-  batch is reproducible and independent of how it is sharded.  Returned tensors are views of the
+  batch is reproducible and independent of how it is sharded.  An episode is a function of its world seed
+  and its actions: set_levels / reset(levels=...) choose the world seeds (fixed evaluation worlds, finite
+  training sets, level-replay curricula, replaying a logged episode).  Returned tensors are views of the
   env's output buffers: they are overwritten by the next `step()` / `reset()`; clone to keep them.
   """
 
@@ -213,7 +251,9 @@ class Env:
         reset_list=z(B, dtype=torch.int32),
         ep_return=z(B, 2, dtype=torch.float64),
         final_stats=z(B, 42, dtype=torch.int32),
-        balance_list=z(B, dtype=torch.int32))
+        balance_list=z(B, dtype=torch.int32),
+        level=torch.full((B,), -1, dtype=torch.int32, device=self._device),  # set_levels
+        final_world_seed=z(B, dtype=torch.int32))
     counters = z(4, dtype=torch.int32)  # adjacent, so the step graph clears both with one memset
     self._state['reset_count'] = counters[0:1]
     self._state['balance_count'] = counters[1:2]
@@ -235,6 +275,8 @@ class Env:
     self._zero_reward = z(B, dtype=torch.float32)  # reward=False (env.py:116-117); info['reward'] keeps the real one
     self._done = z(B, dtype=torch.bool)
     self._actions = z(B, dtype=torch.int32)
+    self._level_in = z(B, dtype=torch.int32)  # set_levels' argument on the device
+    self._level_mask = z(B, dtype=torch.uint8)
 
   def _create(self, size):
     t = tables_lib.render_tables(tuple(int(v) for v in self._view), size)
@@ -322,8 +364,9 @@ class Env:
     torch.cuda.current_stream(self._device).wait_stream(self._stream)
 
   # ---- Env.reset (env.py:70-81) ---------------------------------------------------------------
-  def reset(self, mask=None):
-    """Start a new episode in every env (or in those where `mask` is True); returns obs."""
+  def reset(self, mask=None, levels=None):
+    """Start a new episode in every env (or in those where `mask` is True); returns obs.  With `levels`, this
+    is set_levels(levels, mask) followed by the reset: the episodes it starts play those levels."""
     with torch.cuda.device(self._device):
       ptr = None
       if mask is not None:
@@ -332,6 +375,8 @@ class Env:
         if self._needs_reset and not bool(mask.all()):
           raise RuntimeError('the first reset() must cover every env (envs outside the mask have no world yet)')
         ptr = mask.data_ptr()
+      if levels is not None:
+        self.set_levels(levels, mask)
       s = self._enter()
       if self._observation == 'semantic':  # no frame: the windows of the state the reset left
         _cabi.check(self._lib.cr_reset(self._handle, ptr, None, s))
@@ -344,6 +389,39 @@ class Env:
       self._exit()
     self._needs_reset = False
     return self._out
+
+  # ---- levels ---------------------------------------------------------------------------------
+  def set_levels(self, levels, mask=None):
+    """Choose the world of each env's next episodes (semantics: include/crafter_b200.h, cr_set_levels).
+
+    levels  int tensor / array of shape (num_envs,): -1 = the reference's sequence (episode e of env i plays
+            world seed hash((seed + env_offset + i, e)) % (2**31 - 1)), or a world seed s in [0, 2**31 - 2]:
+            every episode of that env that starts from now on plays world s, exactly the reference's
+            World.reset(seed=s) + generate_world, until the level changes again (auto-reset replays it).
+    mask    bool (num_envs,) or None (all): entries of `levels` outside the mask are ignored.
+
+    The running episodes are left alone; the last assignment before an episode starts wins.  With auto_reset,
+    call it at any time and the new level takes effect from each env's next episode (its world is generated
+    once, now); reset(mask, levels) right after a step starts the new level at once, at the price of
+    generating the worlds of those envs twice in that step.  Checked on the host (ValueError) before anything
+    is launched."""
+    arr, mask = check_levels(levels, mask, self._num_envs)
+    with torch.cuda.device(self._device):
+      arr = arr.to(self._device)
+      if mask is not None:
+        mask = mask.to(self._device)
+      self._level_in.copy_(arr if mask is None else torch.where(mask, arr, -1))
+      if mask is not None:
+        self._level_mask.copy_(mask)
+      s = self._enter()
+      _cabi.check(self._lib.cr_set_levels(self._handle, None if mask is None else self._level_mask.data_ptr(),
+                                          self._level_in.data_ptr(), s))
+      self._exit()
+
+  @property
+  def levels(self):
+    """A copy of the current level of every env, int32 (num_envs,) (-1: the reference's sequence)."""
+    return self._state['level'].clone()
 
   # ---- Env.step (env.py:83-118) ---------------------------------------------------------------
   def step(self, actions):
@@ -490,6 +568,11 @@ class Env:
     return {k: v.clone() for k, v in self._state.items()}
 
   def load_state_dict(self, sd):
+    # snapshots taken before levels existed: every env on the reference's sequence
+    sd = dict(sd)
+    if 'level' not in sd and 'final_world_seed' not in sd:
+      sd['level'] = torch.full_like(self._state['level'], -1)
+      sd['final_world_seed'] = torch.zeros_like(self._state['final_world_seed'])
     if set(sd) != set(self._state):
       raise ValueError(f'state_dict of another layout (keys differ: {sorted(set(sd) ^ set(self._state))})')
     torch.cuda.synchronize(self._device)

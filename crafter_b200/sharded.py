@@ -39,8 +39,11 @@ class ShardedEnv:
   def __getattr__(self, name):
     return getattr(self.env, name)
 
-  def reset(self, mask=None):
-    return self.env.reset(mask)
+  def reset(self, mask=None, levels=None):
+    """`mask` and `levels` (see Env.reset / Env.set_levels) are the LOCAL shard's, like actions."""
+    if levels is None:  # env factories without levels keep working
+      return self.env.reset(mask)
+    return self.env.reset(mask, levels)
 
   def step(self, actions):
     """`actions` are the LOCAL shard's actions, shape (local_num_envs,)."""

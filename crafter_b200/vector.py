@@ -14,7 +14,8 @@ the next episode), and the terminal transition travels in `info` under gymnasium
 
 (`final_observation` / `_final_observation` are kept as aliases for gymnasium <= 0.29 code.)
 `terminated` = the player died (`discount` 0 in the reference, env.py:105,111), `truncated` = the
-episode hit `length` (the registration's max_episode_steps).  Arrays are torch.cuda tensors unless
+episode hit `length` (the registration's max_episode_steps).  `reset(options={'levels': levels})` (with or
+without 'reset_mask') and `set_levels(levels, mask)` choose the worlds the episodes play (Env.set_levels).  Arrays are torch.cuda tensors unless
 `to_numpy=True`.  With `observation='semantic'` (see `crafter_b200.Env`) the observations, `final_obs`
 included, are the local semantic windows and the spaces say so (`Box(0, 18, (gx, gy), uint8)`); with
 `observation='symbolic'` they are the symbolic vectors (`Box(0, 1, (D,), float32)`).
@@ -126,8 +127,14 @@ class VectorEnv(_Base):
     if seed is not None and int(seed) != self.env._seed:
       raise ValueError('the seed is fixed at construction (per-episode seeds derive from it and the env index); '
                        'make a new VectorEnv to change it')
-    mask = (options or {}).get('reset_mask')  # gymnasium 1.x: partial resets through options
-    return self._out(self.env.reset(mask)), {}
+    options = options or {}
+    mask = options.get('reset_mask')  # gymnasium 1.x: partial resets through options
+    # the world seeds of the episodes this reset starts (Env.set_levels; -1 = the reference's sequence)
+    return self._out(self.env.reset(mask, options.get('levels'))), {}
+
+  def set_levels(self, levels, mask=None):
+    """Env.set_levels: the worlds of the envs' next episodes."""
+    self.env.set_levels(levels, mask)
 
   def step(self, actions):
     obs, reward, done, info = self.env.step(actions)

@@ -19,7 +19,7 @@
 extern "C" {
 #endif
 
-#define CR_ABI_VERSION 5
+#define CR_ABI_VERSION 6
 
 typedef struct cr_handle cr_handle;
 
@@ -87,6 +87,14 @@ typedef struct cr_state {
    * episode, for the envs regenerated inside cr_step_symbolic, taken after the step's balance; rows of other
    * envs are left alone.  [B][D] float32. */
   float *final_symbolic;
+  /* Optional (NULL: off, and cr_set_levels fails): the level of every env, see cr_set_levels.  [B] int32,
+   * -1 = the reference's sequence.  The caller fills it with -1 before cr_create and changes it only through
+   * cr_set_levels. */
+  int32_t *level;
+  /* Optional (NULL: off): the world seed of the episode that ended in the last step that ended one, written
+   * by the tick for the envs that finished (with auto_reset the live PS_WORLD_SEED already belongs to the
+   * next episode when the step returns); rows of other envs are left alone.  [B] int32. */
+  int32_t *final_world_seed;
 } cr_state;
 
 int cr_abi_version(void);
@@ -159,6 +167,22 @@ int cr_local(cr_handle *h, uint8_t *out, void *stream);
 /* The symbolic vector of every env as the state stands (the vector cr_step_symbolic returns): out[B][D]
  * float32.  After cr_reset(h, mask, NULL, s) it gives the first vector of the reset envs. */
 int cr_symbolic(cr_handle *h, float *out, void *stream);
+
+/* Levels: which world each env's episodes play.  The world seed of an episode keys every random draw of it
+ * (terrain, creatures, balance, night noise), so an episode is a function of (world seed, actions).
+ *   level -1 (the default)  episode e of env i plays world seed hash((seed + env_offset + i, e)) % (2**31 - 1),
+ *                           the reference's sequence (env.py:72-74);
+ *   level s in [0, 2**31 - 2]  every episode that starts after the assignment plays world seed s: the
+ *                           reference's World.reset(seed=s) + generate_world, every later draw keyed by s.
+ *                           Sticky: auto-reset replays s until the level changes.
+ * An assignment never touches the running episode; the episode counter (PS_EPISODE) advances either way, so
+ * going back to -1 resumes the reference sequence at the env's next episode number.  The last assignment
+ * before an episode starts wins, even when its world was already prefetched: the envs whose mask byte is
+ * non-zero (mask == NULL: all) take levels[env] (device arrays of B entries; values are not checked here),
+ * and their prefetched next world and seed are generated again for the new level on `stream`.  After it,
+ * cr_reset(h, mask, ...) installs those worlds without generating them again (before the first reset too).
+ * Fails when cr_state.level is NULL. */
+int cr_set_levels(cr_handle *h, const uint8_t *mask, const int32_t *levels, void *stream);
 
 /* After the caller has written `mat` itself (state restore, tests): recount what the library keeps
  * incrementally about the terrain (the per-chunk counts of chunk_cnt; a no-op without that buffer
