@@ -46,7 +46,7 @@ class CrState(ctypes.Structure):
 EXPORTS = ('cr_abi_version', 'cr_last_error', 'cr_create', 'cr_destroy', 'cr_reset', 'cr_step',
            'cr_step_host', 'cr_render', 'cr_render_envs', 'cr_semantic', 'cr_recount', 'cr_launch_count',
            'cr_timing', 'cr_source_hash', 'cr_error_flags', 'cr_step_local', 'cr_local',
-           'cr_step_symbolic', 'cr_symbolic', 'cr_set_levels')
+           'cr_step_symbolic', 'cr_symbolic', 'cr_set_levels', 'cr_set_level_table', 'cr_sample_levels')
 
 _lib = None
 
@@ -72,6 +72,8 @@ def declare(lib, prefix='cr_'):
     lib.cr_symbolic.argtypes = [vp, vp, vp]
     lib.cr_recount.argtypes = [vp, vp]
     lib.cr_set_levels.argtypes = [vp, vp, vp, vp]
+    lib.cr_set_level_table.argtypes = [vp, vp, vp, vp, ctypes.c_int]
+    lib.cr_sample_levels.argtypes = [vp, vp, vp]
     lib.cr_launch_count.argtypes = [vp]
     lib.cr_launch_count.restype = ctypes.c_int64
     lib.cr_error_flags.argtypes = [vp, vp, vp]

@@ -85,7 +85,9 @@ enum PState : int {
 enum ErrBits : int {
   ERR_SLOT_OVERFLOW = 1,   // an object did not fit the slot arena and was dropped (slot_capacity)
   ERR_DAYLIGHT_CLAMP = 2,  // the env's step ran past the daylight table: the last entry is used from there on
+  ERR_LEVEL_TABLE = 4,     // a sampled env was seeded from an empty level table: that episode plays world_seed_of
 };
+constexpr int32_t LEVEL_SAMPLED = -2;  // level[env]: every new episode draws its world from the level table (cr_sample_levels)
 enum FrameFlags : int {
   FRAME_NIGHT = 1,  // the env's next frame is a night frame (engine.py:191): the frame kernel draws those first
   FRAME_FINAL = 2,  // the tick left the env's state final (no balance, no regeneration): k_view prepares its view
@@ -106,7 +108,8 @@ struct alignas(8) Ent {
 };
 
 // ---- keyed counter-based randomness (contract: oracle/keyed_rng.py) -------------------------
-enum Domain : uint32_t { D_SEED = 0, D_WG_MAT, D_WG_OBJ, D_UPDATE, D_BALANCE, D_NOISE };
+enum Domain : uint32_t { D_SEED = 0, D_WG_MAT, D_WG_OBJ, D_UPDATE, D_BALANCE, D_NOISE,
+                         D_LEVEL };  // ctr (0,0,0,0), keyed by world_seed_of: the level table draw (wg_level_draw)
 
 CR_DEV uint32_t mulhi32(uint32_t a, uint32_t b) {
 #ifdef CR_HOSTSIM
@@ -253,8 +256,14 @@ struct State {
   uint8_t *final_semantic; // [B][NC] or null (needs final_obs or final_local): its terminal info['semantic']
   uint8_t *final_local;    // [B][gx][gy] or null: the terminal local semantic window (cr_step_local)
   float *final_symbolic;   // [B][22 gx gy + 22] or null: the terminal symbolic vector (cr_step_symbolic)
-  int32_t *level;          // [B] or null: the world seed every new episode plays, -1 = world_seed_of (cr_set_levels)
+  int32_t *level;          // [B] or null: the world seed every new episode plays, -1 = world_seed_of (cr_set_levels),
+                           // LEVEL_SAMPLED = drawn from the level table (cr_sample_levels)
   int32_t *final_world_seed;  // [B] or null: the world seed of the episode that ended last
+  // the level table (cr_set_level_table; caller-owned, read-only for the kernels), not part of the ABI's cr_state
+  const int32_t *lt_seeds;  // [lt_cap] world seeds, or null: no table
+  const uint32_t *lt_cum;   // [lt_cap] inclusive cumulative weights
+  const int32_t *lt_n;      // [1] entries in use
+  int32_t lt_cap;
 };
 
 CR_DEV uint8_t *next_mat_of(const State &st, const Geom &g, int env) { return st.next_mat + (size_t)env * g.NC; }

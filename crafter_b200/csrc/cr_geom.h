@@ -80,6 +80,7 @@ inline void state_from_abi(const cr_state &s, State &st) {
   st.final_obs = s.final_obs; st.final_semantic = s.final_semantic; st.final_local = s.final_local;
   st.final_symbolic = s.final_symbolic;
   st.level = s.level; st.final_world_seed = s.final_world_seed;
+  st.lt_seeds = nullptr; st.lt_cum = nullptr; st.lt_n = nullptr; st.lt_cap = 0;  // cr_set_level_table
 }
 
 }  // namespace cr

@@ -184,18 +184,27 @@ __global__ void k_fill_list(int B, const uint8_t *__restrict__ mask, int32_t *li
   }
 }
 
-// ---- k_set_levels (cr_set_levels): one thread per env.  A masked env takes its new level; its prefetched
-// world, its promoted seed and its ahead seed were made for the old level and are dropped, and the env joins
-// the reset list, over which the caller then generates the world and the seed after it again.
-__global__ void k_set_levels(int B, State st, const uint8_t *__restrict__ mask, const int32_t *__restrict__ levels) {
-  const int env = blockIdx.x * blockDim.x + threadIdx.x;
-  if (env >= B || (mask && !mask[env])) return;
-  st.level[env] = levels[env];
+// ---- k_set_levels (cr_set_levels), k_sample_levels (cr_sample_levels): one thread per env.  A masked env
+// takes its new level (k_sample_levels: LEVEL_SAMPLED); its prefetched world, its promoted seed and its ahead
+// seed were made for the old level and are dropped, and the env joins the reset list, over which the caller
+// then generates the world and the seed after it again.
+__device__ __forceinline__ void level_assign(const State &st, int env, int32_t level) {
+  st.level[env] = level;
   int32_t *nm = next_meta_of(st, env);
   nm[NM_VALID] = 0;
   nm[NM_SEEDED] = 0;
   nm[NM_AHEAD_VALID] = 0;
   st.reset_list[atomicAdd(st.reset_count, 1)] = env;
+}
+__global__ void k_set_levels(int B, State st, const uint8_t *__restrict__ mask, const int32_t *__restrict__ levels) {
+  const int env = blockIdx.x * blockDim.x + threadIdx.x;
+  if (env >= B || (mask && !mask[env])) return;
+  level_assign(st, env, levels[env]);
+}
+__global__ void k_sample_levels(int B, State st, const uint8_t *__restrict__ mask) {
+  const int env = blockIdx.x * blockDim.x + threadIdx.x;
+  if (env >= B || (mask && !mask[env])) return;
+  level_assign(st, env, LEVEL_SAMPLED);
 }
 
 // World generation runs over a list of envs: the explicit reset list, the default schedule's list

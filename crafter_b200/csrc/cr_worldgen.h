@@ -80,8 +80,44 @@ CR_DEV uint8_t *wg_perm_of(const State &st, int env, int episode) {
   return st.perm + ((size_t)env * 2 + (episode & 1)) * 256;
 }
 
+// The table is written between steps, never by a step: read-only loads.
+#if defined(CR_HOSTSIM) || defined(CR_SIMT)
+template <typename T> CR_DEV T wg_table_load(const T *p) { return *p; }
+#else
+template <typename T> CR_DEV T wg_table_load(const T *p) { return __ldg(p); }
+#endif
+
+// The world seed a sampled env (level LEVEL_SAMPLED) plays in `episode`, drawn from the handle's level table
+// (semantics: include/crafter_b200.h, cr_set_level_table).  Called by all lanes of the warp, which all return
+// the seed.  The draw is keyed by the world seed the reference sequence would have played, so it depends on
+// the global env index and the episode number only; integers throughout, so it is exact.  `empty`: there is
+// no table or its total weight is 0, and the reference sequence's seed is returned.
+// The search for the first entry whose cumulative weight exceeds the draw is the warp's: each round the lanes
+// probe CR_LANES evenly spaced entries of the range and a ballot narrows it (2**20 entries: 5 rounds of
+// independent loads, against 20 dependent ones); with one lane (tests/hostsim) it is a bisection.
+CR_DEV uint32_t wg_level_draw(const Geom &g, const State &st, int env, int episode, int lane, bool &empty) {
+  const uint32_t key = world_seed_of(g.seed + g.env_offset + env, episode);
+  int32_t n = st.lt_seeds ? wg_table_load(st.lt_n) : 0;
+  n = n > st.lt_cap ? st.lt_cap : n;
+  const uint32_t total = n > 0 ? wg_table_load(st.lt_cum + n - 1) : 0u;
+  empty = total == 0;
+  if (empty) return key;
+  Rng rng = rng_ctx(key, D_LEVEL, 0);
+  const uint32_t t = rng_randint(rng, total);  // in [0, total)
+  uint32_t lo = 0, hi = (uint32_t)n - 1;  // the answer lies in [lo, hi]: cum[hi] > t holds
+  while (lo < hi) {
+    const uint32_t step = (hi - lo + CR_LANES) / (CR_LANES + 1);  // >= 1
+    const uint32_t at = lo + ((uint32_t)lane + 1) * step - 1;  // lane l probes lo + (l + 1) step - 1, capped at hi
+    const uint32_t above = cr_ballot(wg_table_load(st.lt_cum + (at < hi ? at : hi)) > t);  // monotone in the lane
+    const uint32_t k = above ? (uint32_t)cr_ffs(above) - 1 : (uint32_t)CR_LANES;  // the first lane above the draw
+    if (k < CR_LANES && lo + (k + 1) * step - 1 < hi) hi = lo + (k + 1) * step - 1;
+    if (k > 0) lo += k * step;  // the probe of lane k - 1, plus one
+  }
+  return (uint32_t)wg_table_load(st.lt_seeds + lo);
+}
+
 CR_DEV void wg_seed(const Geom &g, const State &st, int env, int lane, SeedScratch &S, int ahead) {
-  const int32_t *ps = st.pstate + (size_t)env * PS_COUNT;
+  int32_t *ps = st.pstate + (size_t)env * PS_COUNT;
   int32_t *nm = st.next_meta + (size_t)env * NM_COUNT;
   const bool seeded = !ahead && nm[NM_SEEDED];  // promoted by wg_install_player (uniform across the warp)
   const int episode = ahead ? nm[NM_EPISODE] + 1 : ps[PS_EPISODE] + 1;
@@ -90,10 +126,13 @@ CR_DEV void wg_seed(const Geom &g, const State &st, int env, int lane, SeedScrat
   // Two tables per env, by episode parity: the ahead pass writes the one k_wg_mat is NOT reading, so it
   // runs beside the terrain of the world before it instead of behind it.
   uint8_t *perm = wg_perm_of(st, env, episode);
-  uint32_t ws = 0;
+  const int32_t level = st.level ? st.level[env] : -1;  // cr_set_levels, cr_sample_levels (uniform across the warp)
+  uint32_t ws;
+  bool empty = false;
+  if (level == LEVEL_SAMPLED) ws = wg_level_draw(g, st, env, episode, lane, empty);
+  else ws = level >= 0 ? (uint32_t)level : world_seed_of(g.seed + g.env_offset + env, episode);
   if (lane == 0) {
-    const int32_t level = st.level ? st.level[env] : -1;  // cr_set_levels
-    ws = level >= 0 ? (uint32_t)level : world_seed_of(g.seed + g.env_offset + env, episode);
+    if (empty) cr_atomic_or(reinterpret_cast<uint32_t *>(ps + PS_ERROR), (uint32_t)ERR_LEVEL_TABLE);
     nm[ahead ? NM_AHEAD_EPISODE : NM_EPISODE] = episode;
     nm[ahead ? NM_AHEAD_WORLD_SEED : NM_WORLD_SEED] = (int32_t)ws;
     if (!ahead) nm[NM_SEEDED] = 1;

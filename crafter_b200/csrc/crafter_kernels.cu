@@ -487,6 +487,18 @@ int run_step(cr_handle *h, GraphSlot &gs, const int32_t *actions, uint8_t *obs, 
   return 0;
 }
 
+// behind k_set_levels / k_sample_levels on `s`: the next world of the envs they listed (only_invalid: every
+// listed env was invalidated) and, beside its terrain, the seed of the one after it
+int regenerate_relevelled(cr_handle *h, cudaStream_t s) {
+  CR_CUDA(cudaGetLastError());
+  h->launches += 1;
+  int k;
+  if ((k = launch_worldgen(h, s, h->st.reset_list, h->st.reset_count, 1, 1, 0)) < 0) return k;
+  h->launches += k;
+  CR_CUDA(cudaMemsetAsync(h->st.reset_count, 0, sizeof(int32_t), s));  // zero whenever a step begins
+  return 0;
+}
+
 }  // namespace
 
 // The handle's streams, events and graphs belong to the device that was current in cr_create;
@@ -558,14 +570,31 @@ int cr_set_levels(cr_handle *h, const uint8_t *mask, const int32_t *levels, void
   DeviceGuard on_device(h->device);
   cudaStream_t s = (cudaStream_t)stream;
   k_set_levels<<<(h->g.B + 255) / 256, 256, 0, s>>>(h->g.B, h->st, mask, levels);
-  CR_CUDA(cudaGetLastError());
-  h->launches += 1;
-  // the next world (only_invalid: every listed env was invalidated) and, beside its terrain, the one after it
-  int k;
-  if ((k = launch_worldgen(h, s, h->st.reset_list, h->st.reset_count, 1, 1, 0)) < 0) return k;
-  h->launches += k;
-  CR_CUDA(cudaMemsetAsync(h->st.reset_count, 0, sizeof(int32_t), s));  // zero whenever a step begins
+  return regenerate_relevelled(h, s);
+}
+
+int cr_set_level_table(cr_handle *h, const int32_t *seeds, const uint32_t *cum, const int32_t *n, int cap) {
+  if (!h) return fail_msg("null handle");
+  if (seeds && (!cum || !n || cap < 1)) return fail_msg("cr_set_level_table: seeds without cum, n or a capacity >= 1");
+  DeviceGuard on_device(h->device);
+  h->st.lt_seeds = seeds;
+  h->st.lt_cum = seeds ? cum : nullptr;
+  h->st.lt_n = seeds ? n : nullptr;
+  h->st.lt_cap = seeds ? cap : 0;
+  // the cached step graphs hold a copy of `st` in their kernel nodes: the next step captures them again
+  for (GraphSlot &gs : h->slots)
+    if (gs.exec) { cudaGraphExecDestroy(gs.exec); gs.exec = nullptr; }
   return 0;
+}
+
+int cr_sample_levels(cr_handle *h, const uint8_t *mask, void *stream) {
+  if (!h) return fail_msg("null handle");
+  if (!h->st.level) return fail_msg("cr_sample_levels: the handle has no level buffer (cr_state.level is NULL)");
+  if (!h->st.lt_seeds) return fail_msg("cr_sample_levels: the handle has no level table (cr_set_level_table)");
+  DeviceGuard on_device(h->device);
+  cudaStream_t s = (cudaStream_t)stream;
+  k_sample_levels<<<(h->g.B + 255) / 256, 256, 0, s>>>(h->g.B, h->st, mask);
+  return regenerate_relevelled(h, s);
 }
 
 int cr_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, uint8_t *done,

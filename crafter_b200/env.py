@@ -20,6 +20,8 @@ DiscreteSpace = collections.namedtuple('DiscreteSpace', 'n')  # env.py:18-21 (gy
 BoxSpace = collections.namedtuple('BoxSpace', 'low, high, shape, dtype')
 OBSERVATIONS = ('rgb', 'semantic', 'symbolic')
 MAX_LEVEL = 2 ** 31 - 2  # the largest world seed of the reference, hash(...) % (2**31 - 1) (env.py:74)
+LEVEL_SAMPLED = -2  # Env.levels of an env that draws its worlds from the level table (Env.sample_levels)
+MAX_WEIGHT_TOTAL = 2 ** 32 - 1  # the largest total weight of a level table
 # player.facing as (dx, dy) by the facing index of the player record (objects.py:33-34: left, right, up, down)
 FACING = ((-1, 0), (1, 0), (0, -1), (0, 1))
 # The 22 channels of every window cell of observation='symbolic' (layout: include/crafter_b200.h,
@@ -81,6 +83,54 @@ def check_levels(levels, mask, num_envs):
   if lo < -1 or hi > MAX_LEVEL:
     raise ValueError(f'levels must be -1 or world seeds in [0, {MAX_LEVEL}]')
   return arr, mask
+
+
+def _int_vector(values, name):
+  """`values` as a 1-d int64 tensor (on the device it came on); ValueError for another dtype or shape."""
+  if torch.is_tensor(values):
+    if values.dtype.is_floating_point or values.dtype.is_complex or values.dtype == torch.bool:
+      raise ValueError(f'{name} must be integers, not {values.dtype}')
+    arr = values.to(torch.int64)
+  else:
+    a = np.asarray(values)
+    if a.dtype.kind not in 'iu':
+      raise ValueError(f'{name} must be integers, not {a.dtype}')
+    if a.dtype.kind == 'u' and a.size and int(a.max()) > MAX_WEIGHT_TOTAL:
+      raise ValueError(f'{name} out of range')
+    arr = torch.from_numpy(a.astype(np.int64))
+  if arr.dim() != 1:
+    raise ValueError(f'{name} must have shape (n,), not {tuple(arr.shape)}')
+  return arr
+
+
+def check_level_weights(weights, n):
+  """Level table weights checked on the host (one read when they are on a device): int64 (n,), non-negative
+  integers whose total lies in [1, MAX_WEIGHT_TOTAL].  ValueError otherwise."""
+  arr = _int_vector(weights, 'weights')
+  if tuple(arr.shape) != (n,):
+    raise ValueError(f'weights must have shape ({n},), not {tuple(arr.shape)}')
+  lo, hi = torch.stack([arr.min(), arr.max()]).tolist()
+  if lo < 0 or hi > MAX_WEIGHT_TOTAL:  # (a larger entry could wrap the int64 total around)
+    raise ValueError(f'weights must be integers in [0, {MAX_WEIGHT_TOTAL}]')
+  total = int(arr.sum())
+  if not 1 <= total <= MAX_WEIGHT_TOTAL:
+    raise ValueError(f'the total weight must lie in [1, {MAX_WEIGHT_TOTAL}], not {total}')
+  return arr
+
+
+def check_level_table(seeds, weights=None):
+  """Env.set_level_table's arguments checked on the host: (seeds, weights) as int64 (n,) tensors, n >= 1.
+  ValueError for a non-integer dtype, a wrong shape, a seed outside [0, MAX_LEVEL], a negative weight or a total
+  weight outside [1, MAX_WEIGHT_TOTAL]; weights=None is weight 1 for every seed."""
+  arr = _int_vector(seeds, 'seeds')
+  n = arr.numel()
+  if n < 1:
+    raise ValueError('the level table needs at least one seed')
+  lo, hi = torch.stack([arr.min(), arr.max()]).tolist()
+  if lo < 0 or hi > MAX_LEVEL:
+    raise ValueError(f'seeds must be world seeds in [0, {MAX_LEVEL}]')
+  w = torch.ones(n, dtype=torch.int64) if weights is None else check_level_weights(weights, n)
+  return arr, w
 
 
 class Info(dict):
@@ -170,7 +220,9 @@ class Env:
   Randomness is counter-based (Philox keyed by the per-episode world seed, see DESIGN.md), so a
   batch is reproducible and independent of how it is sharded.  An episode is a function of its world seed
   and its actions: set_levels / reset(levels=...) choose the world seeds (fixed evaluation worlds, finite
-  training sets, level-replay curricula, replaying a logged episode).  Returned tensors are views of the
+  training sets, level-replay curricula, replaying a logged episode); set_level_table / sample_levels make envs
+  draw the world of every new episode from a weighted table of world seeds inside the step, and
+  set_level_weights updates the weights without a host read.  Returned tensors are views of the
   env's output buffers: they are overwritten by the next `step()` / `reset()`; clone to keep them.
   """
 
@@ -219,6 +271,7 @@ class Env:
       self._daylight = self._upload(tables_lib.daylight_table(self._n_daylight))
       self._handle, self._tables = self._create(tuple(int(v) for v in self._size))
     self._aux_handles = {}
+    self._table, self._table_len = None, 0  # set_level_table
     self._needs_reset = True
     # raw addresses of the fixed buffers: the per-step calls below hand them to the C ABI without
     # touching torch again (the library switches to its own device itself, see DeviceGuard)
@@ -405,7 +458,7 @@ class Env:
     once, now); reset(mask, levels) right after a step starts the new level at once, at the price of
     generating the worlds of those envs twice in that step.  Checked on the host (ValueError) before anything
     is launched."""
-    arr, mask = check_levels(levels, mask, self._num_envs)
+    arr, mask = check_levels(levels, mask, self._num_envs)  # (also takes the masked envs out of sampling)
     with torch.cuda.device(self._device):
       arr = arr.to(self._device)
       if mask is not None:
@@ -420,8 +473,92 @@ class Env:
 
   @property
   def levels(self):
-    """A copy of the current level of every env, int32 (num_envs,) (-1: the reference's sequence)."""
+    """A copy of the current level of every env, int32 (num_envs,) (-1: the reference's sequence, -2 =
+    LEVEL_SAMPLED: drawn from the level table, see sample_levels)."""
     return self._state['level'].clone()
+
+  # ---- the level sampler ------------------------------------------------------------------------
+  def set_level_table(self, seeds, weights=None):
+    """The table the sampled envs (sample_levels) draw their worlds from (semantics: include/crafter_b200.h,
+    cr_set_level_table): `seeds` (n,) ints in [0, MAX_LEVEL], `weights` (n,) non-negative ints (None: all 1)
+    whose total lies in [1, 2**32 - 1]; a seed of weight 0 is never drawn.  Every new episode of a sampled env
+    draws one seed with probability weight / total, inside the step: no world is generated twice and the
+    host is not read.  The draw is keyed by (seed + env_offset + env, episode), so a run replays from the
+    seed and the table contents, however the batch is sharded.
+
+    Checked on the host (ValueError); this is the rare call.  Replacing the table later is allowed at any
+    time, with the staleness described under set_level_weights."""
+    seeds, weights = check_level_table(seeds, weights)
+    n = seeds.numel()
+    with torch.cuda.device(self._device):
+      if self._table is None or n > self._table['seeds'].numel():  # the buffers belong to the env; grown, never shrunk
+        z = lambda *shape, dtype: torch.zeros(*shape, dtype=dtype, device=self._device)
+        table = dict(seeds=z(n, dtype=torch.int32), cum=z(n, dtype=torch.int32), n=z(1, dtype=torch.int32),
+                     weights=z(n, dtype=torch.int64))
+        _cabi.check(self._lib.cr_set_level_table(self._handle, table['seeds'].data_ptr(), table['cum'].data_ptr(),
+                                                 table['n'].data_ptr(), n))
+        self._table = table
+      self._table_len = n
+      self._table['n'].fill_(n)
+      self._table['seeds'][:n].copy_(seeds)
+      self._write_weights(weights.to(self._device), n)
+
+  def _write_weights(self, weights, n):
+    """int64 device weights (n,) -> the kept copy and the inclusive cumulative sum as uint32 bit patterns."""
+    self._table['weights'][:n].copy_(weights)
+    cum = torch.cumsum(weights, 0)  # int64: exact
+    self._table['cum'][:n].copy_(cum.view(torch.int32)[0::2])  # the low words (little-endian)
+
+  def set_level_weights(self, weights):
+    """New weights for the seeds of the level table, (n,) non-negative ints: the per-step call of a
+    prioritized-level-replay loop.  A device tensor is only checked for dtype and shape and is not read
+    back: nothing here synchronises, and keeping the total in [1, 2**32 - 1] is the caller's part (a zero
+    total makes the sampled envs play the reference's sequence and raises an error bit that check_errors()
+    reports; a larger total wraps around).  Host arrays are checked like set_level_table's.  Float
+    priorities p in [0, 1] are meant to come in as `(p * 2**24).round().to(torch.int64)`, which keeps the
+    total of up to 255 levels in range; scale down for more.
+
+    Nothing in flight is touched: each env's prefetched next world and the seed prepared for the one after it
+    were drawn from the table as it stood and are played as drawn, so new weights reach an env from its third
+    new episode at the latest -- the price of never generating a world twice.  sample_levels(mask) makes
+    them hold from the very next episode of the masked envs, at the cost of generating those worlds again.
+    Weights need not be rewritten every step: a curriculum that updates them every few steps pays less."""
+    if self._table is None:
+      raise RuntimeError('set_level_weights: no level table (call set_level_table first)')
+    n = self._table_len
+    if torch.is_tensor(weights) and weights.is_cuda:
+      arr = _int_vector(weights, 'weights')
+      if tuple(arr.shape) != (n,):
+        raise ValueError(f'weights must have shape ({n},), not {tuple(arr.shape)}')
+    else:
+      arr = check_level_weights(weights, n)
+    with torch.cuda.device(self._device):
+      self._write_weights(arr.to(self._device), n)
+
+  def sample_levels(self, mask=None):
+    """The envs where `mask` is True (None: all) draw the world of every new episode from the level table
+    (set_level_table), until set_levels puts them on a level (or -1) again; `levels` shows LEVEL_SAMPLED = -2
+    for them.  Like set_levels it leaves the running episodes alone and generates the next world of those
+    envs once, now, from the table as it stands; reset(mask) right after it starts such episodes at once."""
+    if self._table is None:
+      raise RuntimeError('sample_levels: no level table (call set_level_table first)')
+    with torch.cuda.device(self._device):
+      if mask is not None:
+        mask = torch.as_tensor(mask, device=self._device).to(torch.bool)
+        if tuple(mask.shape) != (self._num_envs,):
+          raise ValueError(f'mask must have shape ({self._num_envs},), not {tuple(mask.shape)}')
+        self._level_mask.copy_(mask)
+      s = self._enter()
+      _cabi.check(self._lib.cr_sample_levels(self._handle, None if mask is None else self._level_mask.data_ptr(), s))
+      self._exit()
+
+  @property
+  def level_table(self):
+    """(seeds int32 (n,), weights int64 (n,)) copies of the level table, or None."""
+    if self._table is None:
+      return None
+    n = self._table_len
+    return self._table['seeds'][:n].clone(), self._table['weights'][:n].clone()
 
   # ---- Env.step (env.py:83-118) ---------------------------------------------------------------
   def step(self, actions):
@@ -527,7 +664,8 @@ class Env:
 
   def error_flags(self):
     """OR of the envs' sticky error bits (synchronises): 1 = an object was dropped because the slot
-    arena was full (raise slot_capacity), 2 = an env was stepped past its daylight table."""
+    arena was full (raise slot_capacity), 2 = an env was stepped past its daylight table, 4 = a sampled env
+    was seeded from an empty level table (no table, or a total weight of 0)."""
     flags = ctypes.c_int32(0)
     s = self._enter()
     _cabi.check(self._lib.cr_error_flags(self._handle, ctypes.byref(flags), s))
@@ -544,6 +682,9 @@ class Env:
     if flags & 2:
       raise RuntimeError('crafter_b200: an env was stepped past its daylight table '
                          f'({self._n_daylight} entries); daylight is frozen at the last entry there')
+    if flags & 4:
+      raise RuntimeError('crafter_b200: a sampled env was seeded from an empty level table (total weight 0, or '
+                         'no table); it played the world of the reference sequence instead')
 
   def set_inventory(self, values, env_ids=None):
     """Overwrite inventory entries ({item: amount}), like poking `env._player.inventory` on the

@@ -15,7 +15,9 @@ the next episode), and the terminal transition travels in `info` under gymnasium
 (`final_observation` / `_final_observation` are kept as aliases for gymnasium <= 0.29 code.)
 `terminated` = the player died (`discount` 0 in the reference, env.py:105,111), `truncated` = the
 episode hit `length` (the registration's max_episode_steps).  `reset(options={'levels': levels})` (with or
-without 'reset_mask') and `set_levels(levels, mask)` choose the worlds the episodes play (Env.set_levels).  Arrays are torch.cuda tensors unless
+without 'reset_mask') and `set_levels(levels, mask)` choose the worlds the episodes play (Env.set_levels);
+`set_level_table`, `set_level_weights` and `sample_levels` make envs draw them from a weighted table inside the step
+(Env.set_level_table).  Arrays are torch.cuda tensors unless
 `to_numpy=True`.  With `observation='semantic'` (see `crafter_b200.Env`) the observations, `final_obs`
 included, are the local semantic windows and the spaces say so (`Box(0, 18, (gx, gy), uint8)`); with
 `observation='symbolic'` they are the symbolic vectors (`Box(0, 1, (D,), float32)`).
@@ -135,6 +137,18 @@ class VectorEnv(_Base):
   def set_levels(self, levels, mask=None):
     """Env.set_levels: the worlds of the envs' next episodes."""
     self.env.set_levels(levels, mask)
+
+  def set_level_table(self, seeds, weights=None):
+    """Env.set_level_table: the weighted table of world seeds the sampled envs draw from."""
+    self.env.set_level_table(seeds, weights)
+
+  def set_level_weights(self, weights):
+    """Env.set_level_weights: new weights for the table's seeds (no host read with a device tensor)."""
+    self.env.set_level_weights(weights)
+
+  def sample_levels(self, mask=None):
+    """Env.sample_levels: these envs draw the world of every new episode from the level table."""
+    self.env.sample_levels(mask)
 
   def step(self, actions):
     obs, reward, done, info = self.env.step(actions)

@@ -88,8 +88,8 @@ typedef struct cr_state {
    * envs are left alone.  [B][D] float32. */
   float *final_symbolic;
   /* Optional (NULL: off, and cr_set_levels fails): the level of every env, see cr_set_levels.  [B] int32,
-   * -1 = the reference's sequence.  The caller fills it with -1 before cr_create and changes it only through
-   * cr_set_levels. */
+   * -1 = the reference's sequence, -2 = sampled from the level table (cr_sample_levels).  The caller fills it
+   * with -1 before cr_create and changes it only through cr_set_levels / cr_sample_levels. */
   int32_t *level;
   /* Optional (NULL: off): the world seed of the episode that ended in the last step that ended one, written
    * by the tick for the envs that finished (with auto_reset the live PS_WORLD_SEED already belongs to the
@@ -184,6 +184,48 @@ int cr_symbolic(cr_handle *h, float *out, void *stream);
  * Fails when cr_state.level is NULL. */
 int cr_set_levels(cr_handle *h, const uint8_t *mask, const int32_t *levels, void *stream);
 
+/* The level sampler: new episodes draw their world from a weighted table of world seeds, inside the step.
+ *
+ * A handle may have one level table: n world seeds seeds[i] in [0, 2**31 - 2] with integer weights, held as
+ * the inclusive cumulative sum cum[i] (cum[n - 1] is the total weight T, 1 <= T <= 2**32 - 1).  An env is
+ * either on a level (cr_set_levels: -1 or a seed) or sampled (cr_sample_levels; cr_state.level shows
+ * CR_LEVEL_SAMPLED).  Whenever the world seed of episode e of a sampled env is decided -- global env index
+ * j = seed + env_offset + env -- it is
+ *     key = hash((j, e)) % (2**31 - 1)           the world seed the reference sequence would have played
+ *     w   = word 0 of Philox4x32-10, key (key, 6), counter (0, 0, 0, 0)     (6: the draw domain LEVEL)
+ *     t   = (w * T) >> 32                        in [0, T)
+ *     i   = the number of entries with cum[i] <= t      (entries of weight 0 are never drawn)
+ *     ws  = seeds[i]
+ * and from there on the episode is the level path of cr_set_levels: World.reset(seed=ws) + generate_world,
+ * every later draw keyed by ws, PS_WORLD_SEED / final_world_seed report ws.  The draw is integer-only, so it
+ * is exact; it depends on (j, e) and the table, not on the order of threads or on how a batch is sharded over
+ * handles (every handle registers the same table), and it can be replayed from (seed, table contents).
+ *
+ * cr_set_level_table registers (or, with seeds == NULL, removes) the table: DEVICE buffers seeds int32[cap],
+ * cum uint32[cap], n int32[1] (entries in use, 0 <= *n <= cap; a larger *n is read as cap), caller-owned like
+ * every other buffer and valid until replaced, removed or cr_destroy.  The caller rewrites their contents (the
+ * weights, the seeds, *n) with stream-ordered writes whenever it likes, without another call; the call itself
+ * is only needed when the pointers change (the cached step graphs are captured again at the next step).
+ *
+ * Nothing in flight is touched by a table update.  A world seed is decided up to two episodes before it is
+ * played: beside the terrain of an env's prefetched next world, the seed of the world after it is prepared
+ * ahead.  Both were drawn from the table as it stood and are played as drawn, so new weights reach an env after
+ * at most two of its episodes: they hold from its third new episode at the latest.  This staleness is the
+ * price of never generating a world twice.  A caller that needs the new table at once calls cr_sample_levels
+ * again for those envs, which draws and generates their next worlds again.
+ *
+ * A seed decided for a sampled env while there is no table, *n == 0 or T == 0 is the reference sequence's
+ * (the key above), and the env's sticky error bit 2 (value 4, see cr_error_flags) is raised. */
+#define CR_LEVEL_SAMPLED (-2)
+int cr_set_level_table(cr_handle *h, const int32_t *seeds, const uint32_t *cum, const int32_t *n, int cap);
+
+/* The envs whose mask byte is non-zero (mask == NULL: all) become sampled.  As in cr_set_levels, running
+ * episodes are left alone; the prefetched next world and the seeds of those envs are dropped and generated once
+ * on `stream` from the table as it stands (before the first reset this costs nothing extra: cr_reset installs
+ * those worlds).  cr_set_levels(mask, -1 or s) takes an env out of sampling.  Fails without a level table or
+ * when cr_state.level is NULL. */
+int cr_sample_levels(cr_handle *h, const uint8_t *mask, void *stream);
+
 /* After the caller has written `mat` itself (state restore, tests): recount what the library keeps
  * incrementally about the terrain (the per-chunk counts of chunk_cnt; a no-op without that buffer
  * or with CRAFTER_B200_INCR_CENSUS=0). */
@@ -191,7 +233,8 @@ int cr_recount(cr_handle *h, void *stream);
 
 /* OR of the envs' sticky error bits (pstate column 14) into *flags_host, synchronising the stream:
  * bit 0 an object did not fit the slot arena and was dropped (raise slot_capacity), bit 1 an env's step
- * counter ran past the daylight table (n_daylight entries; the last one is used from there on). */
+ * counter ran past the daylight table (n_daylight entries; the last one is used from there on), bit 2 a sampled
+ * env was seeded from an empty level table (cr_set_level_table) and plays the reference sequence's world. */
 int cr_error_flags(cr_handle *h, int32_t *flags_host, void *stream);
 
 /* Number of kernel launches issued by this handle so far (bench.py's gpu_launches). */
