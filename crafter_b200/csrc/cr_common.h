@@ -264,6 +264,14 @@ struct State {
   const uint32_t *lt_cum;   // [lt_cap] inclusive cumulative weights
   const int32_t *lt_n;      // [1] entries in use
   int32_t lt_cap;
+  // the level cache (cr_set_level_cache; caller-owned), not part of the ABI's cr_state: row i holds the world of
+  // the seed lc_tag[i], generated by cr_fill_level_cache; a world is copied from a row only when the tag matches
+  uint8_t *lc_mat;          // [lc_cap][NC] terrain, as next_mat holds it after k_wg_obj; or null: no cache
+  Ent *lc_ents;             // [lc_cap][CAP] creatures in slots 2 .. n - 1, as next_ents
+  int32_t *lc_meta;         // [lc_cap][2] n (NM_NSLOTS) and NM_VALID (bit 1: slot overflow)
+  int32_t *lc_tag;          // [lc_cap] the world seed the row holds (a negative value: none)
+  int32_t *lc_row;          // [B][2] table entry the world of each episode parity was drawn from, -1: none (k_seed)
+  int32_t lc_cap;
 };
 
 CR_DEV uint8_t *next_mat_of(const State &st, const Geom &g, int env) { return st.next_mat + (size_t)env * g.NC; }

@@ -81,6 +81,8 @@ inline void state_from_abi(const cr_state &s, State &st) {
   st.final_symbolic = s.final_symbolic;
   st.level = s.level; st.final_world_seed = s.final_world_seed;
   st.lt_seeds = nullptr; st.lt_cum = nullptr; st.lt_n = nullptr; st.lt_cap = 0;  // cr_set_level_table
+  st.lc_mat = nullptr; st.lc_ents = nullptr; st.lc_meta = nullptr; st.lc_tag = nullptr; st.lc_row = nullptr;
+  st.lc_cap = 0;  // cr_set_level_cache
 }
 
 }  // namespace cr

@@ -252,7 +252,7 @@ k_wg_mat(Geom g, State st, const int32_t *__restrict__ list, const int32_t *__re
   for (int w = blockIdx.x; w < total; w += gridDim.x) {
     const int r = w / tiles, tile = w - r * tiles;
     const int env = list[r];
-    if (wg_skip(st, env, only_invalid)) continue;  // uniform per CTA
+    if (wg_skip(st, env, only_invalid) || wg_cached_row(st, env) >= 0) continue;  // uniform per CTA; k_wg_obj copies
     if (env != cur) {
       __syncthreads();
       const uint8_t *perm = wg_perm_of(st, env, next_meta_of(st, env)[NM_EPISODE]);
@@ -285,6 +285,11 @@ k_wg_obj(Geom g, State st, const int32_t *__restrict__ list, const int32_t *__re
     const int env = list[r];
     if (wg_skip(st, env, only_invalid)) continue;  // uniform per CTA
     if (tid == 0 && blockIdx.x < 1024) cr_stamp(4096 + 1024 + (int)blockIdx.x, 1);
+    const int row = wg_cached_row(st, env);  // uniform per CTA, and the row k_wg_mat skipped
+    if (row >= 0) {
+      wg_copy_cached(g, st, env, row, tid, OBJ_THREADS);
+      continue;
+    }
     uint8_t *mat = next_mat_of(st, g, env);
     Ent *ents = next_ents_of(st, g, env);
     int32_t *nm = next_meta_of(st, env);
@@ -350,6 +355,56 @@ k_wg_obj(Geom g, State st, const int32_t *__restrict__ list, const int32_t *__re
       nm[NM_VALID] = valid;
     }
     __syncthreads();
+  }
+}
+
+// ---- cr_fill_level_cache: the worlds of level table entries into their cache rows ---------------------
+// A chunk of FILL_ROWS rows at a time, the chunk's rows standing in for envs: k_wg_mat and k_wg_obj run on a copy
+// of the State (fill_state) whose next_mat / next_ents are the chunk's rows and whose perm / next_meta are the
+// fill's scratch, so a cached world is generated by the very code that generates it in the step.
+constexpr int FILL_ROWS = 1024;
+struct FillScratch {  // library-owned, one allocation (crafter_kernels.cu)
+  uint8_t perm[FILL_ROWS][2][256];
+  int32_t meta[FILL_ROWS][NM_COUNT];
+  int32_t list[FILL_ROWS];
+  int32_t count;
+};
+__host__ __device__ inline State fill_state(const Geom &g, const State &st, FillScratch *f, int base) {
+  State fs = st;
+  fs.next_mat = st.lc_mat + (size_t)base * g.NC;
+  fs.next_ents = st.lc_ents + (size_t)base * g.CAP;
+  fs.next_meta = &f->meta[0][0];
+  fs.perm = &f->perm[0][0][0];
+  fs.lc_row = nullptr;  // nothing is copied from the cache while it is filled
+  return fs;
+}
+
+// k_fill_seed: one warp per row of the chunk [base, base + rows).  A row already tagged with its entry's seed is
+// skipped; the others are listed, with the seed and the permutation table (wg_perm) of their world in the scratch.
+__global__ void __launch_bounds__(SEED_WPB * 32)
+k_fill_seed(State st, FillScratch *f, int base, int rows) {
+  __shared__ SeedScratch scratch[SEED_WPB];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int r = blockIdx.x * SEED_WPB + warp; r < rows; r += gridDim.x * SEED_WPB) {
+    const int32_t ws = st.lt_seeds[base + r];
+    if (ws < 0 || st.lc_tag[base + r] == ws) continue;  // uniform per warp
+    if (lane == 0) {
+      f->list[atomicAdd(&f->count, 1)] = r;
+      f->meta[r][NM_EPISODE] = 0;  // perm[r][0]
+      f->meta[r][NM_WORLD_SEED] = ws;
+    }
+    wg_perm((uint32_t)ws, f->perm[r][0], lane, scratch[warp]);
+    __syncwarp();
+  }
+}
+
+// k_fill_tag: behind k_wg_obj, n, NM_VALID and last the tag of every row the chunk generated.
+__global__ void k_fill_tag(State st, const FillScratch *__restrict__ f, int base) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < f->count; i += gridDim.x * blockDim.x) {
+    const int r = f->list[i];
+    st.lc_meta[(size_t)(base + r) * 2] = f->meta[r][NM_NSLOTS];
+    st.lc_meta[(size_t)(base + r) * 2 + 1] = f->meta[r][NM_VALID];
+    st.lc_tag[base + r] = f->meta[r][NM_WORLD_SEED];
   }
 }
 

@@ -95,7 +95,9 @@ template <typename T> CR_DEV T wg_table_load(const T *p) { return __ldg(p); }
 // The search for the first entry whose cumulative weight exceeds the draw is the warp's: each round the lanes
 // probe CR_LANES evenly spaced entries of the range and a ballot narrows it (2**20 entries: 5 rounds of
 // independent loads, against 20 dependent ones); with one lane (tests/hostsim) it is a bisection.
-CR_DEV uint32_t wg_level_draw(const Geom &g, const State &st, int env, int episode, int lane, bool &empty) {
+// `entry` (optional): the index of the drawn entry, left alone when the table is empty.
+CR_DEV uint32_t wg_level_draw(const Geom &g, const State &st, int env, int episode, int lane, bool &empty,
+                              uint32_t *entry = nullptr) {
   const uint32_t key = world_seed_of(g.seed + g.env_offset + env, episode);
   int32_t n = st.lt_seeds ? wg_table_load(st.lt_n) : 0;
   n = n > st.lt_cap ? st.lt_cap : n;
@@ -113,6 +115,7 @@ CR_DEV uint32_t wg_level_draw(const Geom &g, const State &st, int env, int episo
     if (k < CR_LANES && lo + (k + 1) * step - 1 < hi) hi = lo + (k + 1) * step - 1;
     if (k > 0) lo += k * step;  // the probe of lane k - 1, plus one
   }
+  if (entry) *entry = lo;
   return (uint32_t)wg_table_load(st.lt_seeds + lo);
 }
 
@@ -127,15 +130,18 @@ CR_DEV void wg_seed(const Geom &g, const State &st, int env, int lane, SeedScrat
   // runs beside the terrain of the world before it instead of behind it.
   uint8_t *perm = wg_perm_of(st, env, episode);
   const int32_t level = st.level ? st.level[env] : -1;  // cr_set_levels, cr_sample_levels (uniform across the warp)
-  uint32_t ws;
+  uint32_t ws, entry = ~0u;  // entry: the table entry a sampled world was drawn from
   bool empty = false;
-  if (level == LEVEL_SAMPLED) ws = wg_level_draw(g, st, env, episode, lane, empty);
+  if (level == LEVEL_SAMPLED) ws = wg_level_draw(g, st, env, episode, lane, empty, &entry);
   else ws = level >= 0 ? (uint32_t)level : world_seed_of(g.seed + g.env_offset + env, episode);
   if (lane == 0) {
     if (empty) cr_atomic_or(reinterpret_cast<uint32_t *>(ps + PS_ERROR), (uint32_t)ERR_LEVEL_TABLE);
     nm[ahead ? NM_AHEAD_EPISODE : NM_EPISODE] = episode;
     nm[ahead ? NM_AHEAD_WORLD_SEED : NM_WORLD_SEED] = (int32_t)ws;
     if (!ahead) nm[NM_SEEDED] = 1;
+    // the level cache row that may hold this world, by episode parity like perm (-1: none); only a hint, the
+    // world is copied only if the row's tag is ws when it is built (wg_cached_row)
+    if (st.lc_row) st.lc_row[(size_t)env * 2 + (episode & 1)] = (int32_t)entry;
   }
   wg_perm(ws, perm, lane, S);  // only lane 0 uses `ws`
   if (ahead && lane == 0) nm[NM_AHEAD_VALID] = 1;
@@ -373,6 +379,42 @@ CR_DEV void wg_material_tile(const Geom &g, const NoiseTables &t, uint32_t world
     const uint8_t m = T.result[c];
     const int type = wg_object(g, world_seed, x, y, m);
     out[cell] = (uint8_t)(m | ((type ? type - 1 : 0) << OBJ_SHIFT));
+  }
+}
+
+// ---- the level cache (semantics: include/crafter_b200.h, cr_set_level_cache) --------------------
+// The cache row holding the world about to be built into the env's next_* buffers (the one of next_meta's
+// NM_EPISODE / NM_WORLD_SEED), or -1: the row k_seed recorded for that episode's parity, if it lies in the cache
+// and its tag is the world's seed.  The same answer in every thread that asks within one step.
+CR_DEV int wg_cached_row(const State &st, int env) {
+  if (!st.lc_row) return -1;
+  const int32_t *nm = next_meta_of(st, env);
+  const int32_t row = st.lc_row[(size_t)env * 2 + (nm[NM_EPISODE] & 1)];
+  return row >= 0 && row < st.lc_cap && st.lc_tag[row] == nm[NM_WORLD_SEED] ? row : -1;
+}
+
+// What k_wg_mat and k_wg_obj would write for the world of cache row `row`, copied from the row instead (all
+// `nthreads` threads): the terrain, the creatures in slots 2 .. n - 1, n and NM_VALID with its overflow bit.
+CR_DEV void wg_copy_cached(const Geom &g, const State &st, int env, int row, int tid, int nthreads) {
+  const uint8_t *src = st.lc_mat + (size_t)row * g.NC;
+  uint8_t *mat = next_mat_of(st, g, env);
+  if ((g.NC & 15) == 0) {  // rows of every env and of every cache row stay 16-byte aligned
+    const uint64_t *s8 = reinterpret_cast<const uint64_t *>(src);
+    uint64_t *d8 = reinterpret_cast<uint64_t *>(mat);
+    for (int i = tid; i < g.NC / 8; i += nthreads) d8[i] = s8[i];
+  } else {
+    for (int c = tid; c < g.NC; c += nthreads) mat[c] = src[c];
+  }
+  const int32_t *meta = st.lc_meta + (size_t)row * 2;
+  const int n = imin(meta[0], g.CAP);
+  const Ent *se = st.lc_ents + (size_t)row * g.CAP;
+  Ent *ents = next_ents_of(st, g, env);
+  for (int s = 2 + tid; s < n; s += nthreads) ents[s] = se[s];
+  cr_syncblock();  // every thread has looked at NM_VALID (wg_skip) before it changes
+  if (tid == 0) {
+    int32_t *nm = next_meta_of(st, env);
+    nm[NM_NSLOTS] = n;
+    nm[NM_VALID] = 1 | (meta[1] & 2);
   }
 }
 

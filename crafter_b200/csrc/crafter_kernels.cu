@@ -135,6 +135,7 @@ struct cr_handle {
   float *d2h_reward;
   uint8_t *d2h_done;
   int32_t *err_word;  // cr_error_flags' reduction target
+  FillScratch *fill;  // cr_fill_level_cache's scratch, allocated by its first call
 };
 
 namespace {
@@ -367,6 +368,7 @@ void destroy_handle(cr_handle *h) {
     for (int j = 0; j < 2; ++j)
       if (h->t_ev[i][j]) cudaEventDestroy(h->t_ev[i][j]);
   if (h->err_word) cudaFree(h->err_word);
+  if (h->fill) cudaFree(h->fill);
   if (h->st.frame_order) cudaFree(h->st.frame_order);
   free(h);
 }
@@ -600,6 +602,53 @@ int cr_sample_levels(cr_handle *h, const uint8_t *mask, void *stream) {
   cudaStream_t s = (cudaStream_t)stream;
   k_sample_levels<<<(h->g.B + 255) / 256, 256, 0, s>>>(h->g.B, h->st, mask);
   return regenerate_relevelled(h, s);
+}
+
+int cr_set_level_cache(cr_handle *h, uint8_t *mat, void *ents, int32_t *meta, int32_t *tag, int32_t *row, int cap) {
+  if (!h) return fail_msg("null handle");
+  if (mat && (!ents || !meta || !tag || !row || cap < 1))
+    return fail_msg("cr_set_level_cache: mat without ents, meta, tag, row or a capacity >= 1");
+  DeviceGuard on_device(h->device);
+  h->st.lc_mat = mat;
+  h->st.lc_ents = mat ? (Ent *)ents : nullptr;
+  h->st.lc_meta = mat ? meta : nullptr;
+  h->st.lc_tag = mat ? tag : nullptr;
+  h->st.lc_row = mat ? row : nullptr;
+  h->st.lc_cap = mat ? cap : 0;
+  for (GraphSlot &gs : h->slots)  // (as cr_set_level_table: the graphs hold a copy of `st`)
+    if (gs.exec) { cudaGraphExecDestroy(gs.exec); gs.exec = nullptr; }
+  return 0;
+}
+
+int cr_fill_level_cache(cr_handle *h, int first, int count, void *stream) {
+  if (!h) return fail_msg("null handle");
+  if (!h->st.lt_seeds) return fail_msg("cr_fill_level_cache: the handle has no level table (cr_set_level_table)");
+  if (!h->st.lc_mat) return fail_msg("cr_fill_level_cache: the handle has no level cache (cr_set_level_cache)");
+  if (first < 0 || count < 0) return fail_msg("cr_fill_level_cache: negative first or count");
+  DeviceGuard on_device(h->device);
+  cudaStream_t s = (cudaStream_t)stream;
+  const Geom &g = h->g;
+  const long long cap = h->st.lt_cap < h->st.lc_cap ? h->st.lt_cap : h->st.lc_cap;
+  const long long end = (long long)first + count < cap ? (long long)first + count : cap;
+  if (first >= end) return 0;
+  if (!h->fill) CR_CUDA(cudaMalloc(&h->fill, sizeof(FillScratch)));  // library-owned, like err_word
+  const int tiles = (g.NC + WG_CELLS - 1) / WG_CELLS;
+  for (long long base = first; base < end; base += FILL_ROWS) {
+    const int rows = (int)(end - base < FILL_ROWS ? end - base : FILL_ROWS);
+    const State fs = fill_state(g, h->st, h->fill, (int)base);
+    const int32_t *list = h->fill->list, *n = &h->fill->count;
+    CR_CUDA(cudaMemsetAsync(&h->fill->count, 0, sizeof(int32_t), s));
+    k_fill_seed<<<(rows + SEED_WPB - 1) / SEED_WPB, SEED_WPB * 32, 0, s>>>(h->st, h->fill, (int)base, rows);
+    const long long want = (long long)rows * tiles;
+    const int mat_grid = (int)(want < (long long)h->num_sms * 16 ? want : (long long)h->num_sms * 16);
+    CR_LAUNCH(k_wg_mat, h->is_default, mat_grid, WG_THREADS, 0, s, g, fs, list, n, 0);
+    CR_LAUNCH(k_wg_obj, h->is_default, rows < h->num_sms * 2 ? rows : h->num_sms * 2, OBJ_THREADS, 0, s, g, fs, list, n,
+              0);
+    k_fill_tag<<<(rows + 255) / 256, 256, 0, s>>>(h->st, h->fill, (int)base);
+    CR_CUDA(cudaGetLastError());
+    h->launches += 4;
+  }
+  return 0;
 }
 
 int cr_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, uint8_t *done,

@@ -279,6 +279,7 @@ class Env:
       self._handle, self._tables = self._create(tuple(int(v) for v in self._size))
     self._aux_handles = {}
     self._table, self._table_len = None, 0  # set_level_table
+    self._cache = None  # set_level_cache
     self._needs_reset = True
     # raw addresses of the fixed buffers: the per-step calls below hand them to the C ABI without
     # touching torch again (the library switches to its own device itself, see DeviceGuard)
@@ -516,6 +517,8 @@ class Env:
       self._table['n'].fill_(n)
       self._table['seeds'][:n].copy_(seeds)
       self._write_weights(weights.to(self._device), n)
+      if self._cache is not None:  # new rows for a grown table; only the rows whose seed changed are generated
+        self._fill_level_cache()
 
   def _write_weights(self, weights, n):
     """int64 device weights (n,) -> the kept copy and the inclusive cumulative sum as uint32 bit patterns."""
@@ -573,6 +576,63 @@ class Env:
       return None
     n = self._table_len
     return self._table['seeds'][:n].clone(), self._table['weights'][:n].clone()
+
+  # ---- the level cache ------------------------------------------------------------------------------
+  def set_level_cache(self, enabled=True):
+    """Keep the world of every level table entry generated on the device, so that sampled envs copy their next
+    world instead of generating it (semantics: include/crafter_b200.h, cr_set_level_cache).  Every output and
+    the state stay bit-identical to a run without the cache; only time and memory change.
+
+    enabled=True allocates one row per entry of the table's buffers and generates the worlds, on the caller's
+    stream; later set_level_table calls generate only the rows whose seed changed (and add rows when the table
+    grows); set_level_weights never touches the cache.  enabled=False frees the rows.  The memory is
+    level_cache['bytes']: about 6.2 KB per world at area 64 x 64 (slot capacity 256), about 96 KB at 256 x 256;
+    a table of 2**20 seeds at the default geometry takes about 6.5 GB.  Envs on level -1 or a fixed level are
+    not cached."""
+    if not enabled:
+      if self._cache is not None:
+        _cabi.check(self._lib.cr_set_level_cache(self._handle, None, None, None, None, None, 0))
+        self._cache = None
+      return
+    if self._table is None:
+      raise RuntimeError('set_level_cache: no level table (call set_level_table first)')
+    with torch.cuda.device(self._device):
+      self._fill_level_cache()
+
+  def _fill_level_cache(self):
+    """(Re)register rows for every entry of the table's buffers, grown with the table (the rows held so far are
+    kept), and generate the worlds of the entries in use whose row does not hold their seed."""
+    rows = self._table['seeds'].numel()
+    old = self._cache
+    if old is None or old['tag'].numel() < rows:
+      z = lambda *shape, dtype: torch.zeros(*shape, dtype=dtype, device=self._device)
+      cache = dict(mat=z(rows, self._area[0] * self._area[1], dtype=torch.uint8),
+                   ents=z(rows, self._capacity, dtype=torch.int64), meta=z(rows, 2, dtype=torch.int32),
+                   tag=torch.full((rows,), -1, dtype=torch.int32, device=self._device),
+                   row=old['row'] if old else torch.full((self._num_envs, 2), -1, dtype=torch.int32, device=self._device))
+      if old is not None:  # (the last fill ran on the env's stream, which _exit() made this stream wait for)
+        for k in ('mat', 'ents', 'meta', 'tag'):
+          cache[k][:old[k].shape[0]].copy_(old[k])
+      for v in cache.values():  # read by the env's stream: not reused by torch before that stream is done
+        v.record_stream(self._stream)
+      _cabi.check(self._lib.cr_set_level_cache(self._handle, *(cache[k].data_ptr() for k in (
+          'mat', 'ents', 'meta', 'tag', 'row')), rows))
+      self._cache = cache
+    s = self._enter()
+    _cabi.check(self._lib.cr_fill_level_cache(self._handle, 0, self._table_len, s))
+    self._exit()
+
+  @property
+  def level_cache(self):
+    """None without a level cache, else {'rows': worlds it can hold, 'bytes_per_world', 'bytes': all of it}
+    (set_level_cache states the sizes)."""
+    if self._cache is None:
+      return None
+    c = self._cache
+    rows = c['tag'].numel()
+    per_world = sum(c[k].element_size() * c[k][0].numel() for k in ('mat', 'ents', 'meta', 'tag'))
+    return dict(rows=rows, bytes_per_world=per_world,
+                bytes=per_world * rows + c['row'].element_size() * c['row'].numel())
 
   # ---- Env.step (env.py:83-118) ---------------------------------------------------------------
   def step(self, actions):

@@ -150,6 +150,10 @@ class VectorEnv(_Base):
     """Env.sample_levels: these envs draw the world of every new episode from the level table."""
     self.env.sample_levels(mask)
 
+  def set_level_cache(self, enabled=True):
+    """Env.set_level_cache: keep the level table's worlds generated on the device (memory for time)."""
+    self.env.set_level_cache(enabled)
+
   def step(self, actions):
     obs, reward, done, info = self.env.step(actions)
     dead = self.env.state['final_stats'][:, 23] != 0

@@ -5,7 +5,8 @@
  * (crafter/env.py:25).  Each entry point below names the reference interface it replaces.  All
  * buffers are owned by the caller (torch tensors on the Python side) and passed as raw device
  * pointers; the library allocates no device memory (it owns a few auxiliary CUDA streams and events
- * per handle for the branches of the step graph, and one 4-byte word for cr_error_flags), starts no threads and is stream-ordered.
+ * per handle for the branches of the step graph, one 4-byte word for cr_error_flags and the scratch of
+ * cr_fill_level_cache), starts no threads and is stream-ordered.
  * Every function returns 0 on success and a negative code on error; cr_last_error() describes the
  * last failure of the calling thread.  A handle is bound to the device that was current in cr_create and is not re-entrant;
  * every entry point switches to that device for the duration of the call when another is current.
@@ -245,6 +246,43 @@ int cr_set_level_table(cr_handle *h, const int32_t *seeds, const uint32_t *cum, 
  * those worlds).  cr_set_levels(mask, -1 or s) takes an env out of sampling.  Fails without a level table or
  * when cr_state.level is NULL. */
 int cr_sample_levels(cr_handle *h, const uint8_t *mask, void *stream);
+
+/* The level cache: sampled envs copy their next world from pre-generated worlds of the level table instead of
+ * generating it.  A memory-for-time trade the caller opts into; the results are the same bit for bit.
+ *
+ * A handle with a level table may have one cache of `cap` rows, row i for table entry i.  A row holds a world --
+ * the terrain (next_mat after generation), the creature slots [2, n) (next_ents), n, and the slot-overflow bit
+ * (cr_error_flags bit 0 at install) -- and a tag, the world seed the row holds.  The world of seed s is a function
+ * of s and the geometry, so a row tagged s holds exactly what generating s gives.
+ *   - Sampled envs decide their world seeds exactly as without a cache (the draw and the staleness of
+ *     cr_set_level_table are unchanged).  k_seed notes the entry i a world was drawn from; when the step that
+ *     builds the env's next world finds row i tagged with the drawn seed, the world is copied from the row and its
+ *     terrain and creature passes are skipped.  Any other case -- the caller rewrote seeds[i] after the fill, the
+ *     row was never filled, the table or the cache was replaced after the draw -- generates the world as before.
+ *     So a run with a cache is bit-identical to the same run without one, in every output and in all of cr_state
+ *     (the permutation table `perm` is still computed for every world); only time and memory differ.
+ *   - Envs on level -1 or on a fixed level generate their worlds as without a cache.
+ *
+ * cr_set_level_cache registers (or, with mat == NULL, removes) the cache: caller-owned DEVICE buffers, valid until
+ * replaced, removed or cr_destroy:
+ *   mat   uint8[cap][area_w * area_h]      terrain of each row
+ *   ents  8-byte records [cap][slot_capacity]   its creatures (slots 2 .. n - 1)
+ *   meta  int32[cap][2]                    n, and 1 | 2 * (slot overflow)
+ *   tag   int32[cap]                       the seed the row holds; fill with -1 (any negative value: none)
+ *   row   int32[num_envs][2]               scratch of k_seed: the entry each env's world of an episode parity was
+ *                                          drawn from (any initial contents are harmless: only a tag match counts)
+ * No stream: like cr_set_level_table it changes pointers only (the cached step graphs are captured again at the
+ * next step).  Rows are filled by cr_fill_level_cache and by nothing else; a caller may write tags itself (-1
+ * empties a row).
+ *
+ * cr_fill_level_cache generates, on `stream`, the worlds of seeds[first, first + count) of the registered table
+ * into their rows and tags them, skipping the rows already tagged with their entry's seed (entries at or beyond
+ * either capacity are ignored; the table's *n is not looked at).  It reads the table and writes the cache and
+ * nothing else: no live or prefetched state of the envs.  Its scratch is library-owned: about 0.56 MB, allocated
+ * by the first call and freed by cr_destroy.  Fails without a table or a cache.  Sizes: a row is W*H + 8 *
+ * slot_capacity + 12 bytes, 6,156 at the default geometry (64 x 64, slot_capacity 256). */
+int cr_set_level_cache(cr_handle *h, uint8_t *mat, void *ents, int32_t *meta, int32_t *tag, int32_t *row, int cap);
+int cr_fill_level_cache(cr_handle *h, int first, int count, void *stream);
 
 /* After the caller has written `mat` itself (state restore, tests): recount what the library keeps
  * incrementally about the terrain (the per-chunk counts of chunk_cnt; a no-op without that buffer
