@@ -184,8 +184,9 @@ __global__ void k_fill_list(int B, const uint8_t *__restrict__ mask, int32_t *li
   }
 }
 
-// ---- k_set_levels (cr_set_levels), k_sample_levels (cr_sample_levels): one thread per env.  A masked env
-// takes its new level (k_sample_levels: LEVEL_SAMPLED); its prefetched world, its promoted seed and its ahead
+// ---- k_set_levels (cr_set_levels), k_sample_levels (cr_sample_levels), k_pin_levels (cr_pin_levels): one thread
+// per env.  A masked env takes its new level (k_sample_levels: LEVEL_SAMPLED; k_pin_levels: LEVEL_PINNED_BASE -
+// entry, and a negative entry pins the env to no entry); its prefetched world, its promoted seed and its ahead
 // seed were made for the old level and are dropped, and the env joins the reset list, over which the caller
 // then generates the world and the seed after it again.
 __device__ __forceinline__ void level_assign(const State &st, int env, int32_t level) {
@@ -205,6 +206,12 @@ __global__ void k_sample_levels(int B, State st, const uint8_t *__restrict__ mas
   const int env = blockIdx.x * blockDim.x + threadIdx.x;
   if (env >= B || (mask && !mask[env])) return;
   level_assign(st, env, LEVEL_SAMPLED);
+}
+__global__ void k_pin_levels(int B, State st, const uint8_t *__restrict__ mask, const int32_t *__restrict__ entries) {
+  const int env = blockIdx.x * blockDim.x + threadIdx.x;
+  if (env >= B || (mask && !mask[env])) return;
+  const int32_t e = entries[env];
+  level_assign(st, env, e >= 0 ? LEVEL_PINNED_BASE - e : INT32_MIN);  // INT32_MIN: entry 2**31 - 3, never in a table
 }
 
 // World generation runs over a list of envs: the explicit reset list, the default schedule's list

@@ -119,6 +119,18 @@ CR_DEV uint32_t wg_level_draw(const Geom &g, const State &st, int env, int episo
   return (uint32_t)wg_table_load(st.lt_seeds + lo);
 }
 
+// The world seed an env pinned to table entry e (cr_pin_levels) plays in `episode`: seeds[e] when e lies below the
+// table's *n (and its capacity), else, like an empty table, the reference sequence's seed with `empty` set.
+CR_DEV uint32_t wg_level_pinned(const Geom &g, const State &st, int env, int episode, int32_t e, bool &empty,
+                                uint32_t &entry) {
+  int32_t n = st.lt_seeds ? wg_table_load(st.lt_n) : 0;
+  n = n > st.lt_cap ? st.lt_cap : n;
+  empty = e >= n;
+  if (empty) return world_seed_of(g.seed + g.env_offset + env, episode);
+  entry = (uint32_t)e;
+  return (uint32_t)wg_table_load(st.lt_seeds + e);
+}
+
 CR_DEV void wg_seed(const Geom &g, const State &st, int env, int lane, SeedScratch &S, int ahead) {
   int32_t *ps = st.pstate + (size_t)env * PS_COUNT;
   int32_t *nm = st.next_meta + (size_t)env * NM_COUNT;
@@ -129,10 +141,11 @@ CR_DEV void wg_seed(const Geom &g, const State &st, int env, int lane, SeedScrat
   // Two tables per env, by episode parity: the ahead pass writes the one k_wg_mat is NOT reading, so it
   // runs beside the terrain of the world before it instead of behind it.
   uint8_t *perm = wg_perm_of(st, env, episode);
-  const int32_t level = st.level ? st.level[env] : -1;  // cr_set_levels, cr_sample_levels (uniform across the warp)
-  uint32_t ws, entry = ~0u;  // entry: the table entry a sampled world was drawn from
+  const int32_t level = st.level ? st.level[env] : -1;  // cr_set/sample/pin_levels (uniform across the warp)
+  uint32_t ws, entry = ~0u;  // entry: the table entry a sampled or pinned world was taken from
   bool empty = false;
   if (level == LEVEL_SAMPLED) ws = wg_level_draw(g, st, env, episode, lane, empty, &entry);
+  else if (level <= LEVEL_PINNED_BASE) ws = wg_level_pinned(g, st, env, episode, LEVEL_PINNED_BASE - level, empty, entry);
   else ws = level >= 0 ? (uint32_t)level : world_seed_of(g.seed + g.env_offset + env, episode);
   if (lane == 0) {
     if (empty) cr_atomic_or(reinterpret_cast<uint32_t *>(ps + PS_ERROR), (uint32_t)ERR_LEVEL_TABLE);

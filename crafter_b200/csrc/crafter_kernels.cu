@@ -41,6 +41,7 @@
 #include "cr_update.h"
 #include "cr_worldgen.h"
 #include "cr_kernels.h"
+#include "cr_author.h"
 
 using namespace cr;
 using namespace cr::kernels;
@@ -136,6 +137,8 @@ struct cr_handle {
   uint8_t *d2h_done;
   int32_t *err_word;  // cr_error_flags' reduction target
   FillScratch *fill;  // cr_fill_level_cache's scratch, allocated by its first call
+  int32_t *author;    // cr_author_levels' scratch (author_words(author_cap) int32), allocated and grown by it
+  int author_cap;
 };
 
 namespace {
@@ -369,6 +372,7 @@ void destroy_handle(cr_handle *h) {
       if (h->t_ev[i][j]) cudaEventDestroy(h->t_ev[i][j]);
   if (h->err_word) cudaFree(h->err_word);
   if (h->fill) cudaFree(h->fill);
+  if (h->author) cudaFree(h->author);
   if (h->st.frame_order) cudaFree(h->st.frame_order);
   free(h);
 }
@@ -649,6 +653,50 @@ int cr_fill_level_cache(cr_handle *h, int first, int count, void *stream) {
     h->launches += 4;
   }
   return 0;
+}
+
+int cr_author_levels(cr_handle *h, const int32_t *entries, const uint8_t *worlds, int count, int32_t *status,
+                     void *stream) {
+  if (!h) return fail_msg("null handle");
+  if (!h->st.lt_seeds) return fail_msg("cr_author_levels: the handle has no level table (cr_set_level_table)");
+  if (!h->st.lc_mat) return fail_msg("cr_author_levels: the handle has no level cache (cr_set_level_cache)");
+  if (count < 0) return fail_msg("cr_author_levels: negative count");
+  if (count == 0) return 0;
+  if (!entries || !worlds || !status) return fail_msg("null argument");
+  DeviceGuard on_device(h->device);
+  cudaStream_t s = (cudaStream_t)stream;
+  const Geom &g = h->g;
+  const int cap = h->st.lt_cap < h->st.lc_cap ? h->st.lt_cap : h->st.lc_cap;
+  if (h->author_cap < cap) {  // grown with the table and the cache, never shrunk; the claims start out free (-1)
+    if (h->author) CR_CUDA(cudaFree(h->author));
+    h->author = nullptr;
+    h->author_cap = 0;
+    CR_CUDA(cudaMalloc(&h->author, author_words(cap) * sizeof(int32_t)));
+    h->author_cap = cap;
+    CR_CUDA(cudaMemsetAsync(author_claim(h->author), 0xFF, (size_t)cap * sizeof(int32_t), s));
+  }
+  int32_t *scratch = h->author;
+  CR_CUDA(cudaMemsetAsync(scratch, 0, 2 * sizeof(int32_t), s));
+  CR_CUDA(cudaMemsetAsync(status, 0, (size_t)count * sizeof(int32_t), s));
+  k_author_check<<<count, AUTHOR_THREADS, 0, s>>>(g, h->st, entries, worlds, cap, status, scratch);
+  k_author_copy<<<count, AUTHOR_THREADS, 0, s>>>(g, h->st, entries, worlds, count, scratch);
+  const State as = author_state(h->st, scratch, h->author_cap);
+  CR_LAUNCH(k_wg_obj, h->is_default, count < h->num_sms * 2 ? count : h->num_sms * 2, OBJ_THREADS, 0, s, g, as, entries,
+            scratch + 1, 0);
+  k_author_tag<<<(count + 255) / 256, 256, 0, s>>>(h->st, entries, count, cap, scratch, h->author_cap);
+  CR_CUDA(cudaGetLastError());
+  h->launches += 4;
+  return 0;
+}
+
+int cr_pin_levels(cr_handle *h, const uint8_t *mask, const int32_t *entries, void *stream) {
+  if (!h || !entries) return fail_msg("null argument");
+  if (!h->st.level) return fail_msg("cr_pin_levels: the handle has no level buffer (cr_state.level is NULL)");
+  if (!h->st.lt_seeds) return fail_msg("cr_pin_levels: the handle has no level table (cr_set_level_table)");
+  DeviceGuard on_device(h->device);
+  cudaStream_t s = (cudaStream_t)stream;
+  k_pin_levels<<<(h->g.B + 255) / 256, 256, 0, s>>>(h->g.B, h->st, mask, entries);
+  return regenerate_relevelled(h, s);
 }
 
 int cr_step(cr_handle *h, const int32_t *actions, uint8_t *obs, float *reward, uint8_t *done,

@@ -21,6 +21,13 @@ BoxSpace = collections.namedtuple('BoxSpace', 'low, high, shape, dtype')
 OBSERVATIONS = ('rgb', 'semantic', 'symbolic')
 MAX_LEVEL = 2 ** 31 - 2  # the largest world seed of the reference, hash(...) % (2**31 - 1) (env.py:74)
 LEVEL_SAMPLED = -2  # Env.levels of an env that draws its worlds from the level table (Env.sample_levels)
+LEVEL_PINNED_BASE = -3  # Env.levels of an env pinned to table entry e is LEVEL_PINNED_BASE - e (Env.pin_levels)
+# cr_author_levels' status bits (include/crafter_b200.h): why a world was rejected
+AUTHOR_REASONS = ((1, 'a byte out of range (material outside 1..12 or creature outside 0..3)'),
+                  (2, 'a creature on a cell that is not grass, sand or path'),
+                  (4, 'the start cell (W/2, H/2) is not grass, sand or path, or holds a creature'),
+                  (8, 'more than slot_capacity - 2 creatures'),
+                  (16, 'the entry lies outside the cache, or appears twice in the call'))
 MAX_WEIGHT_TOTAL = 2 ** 32 - 1  # the largest total weight of a level table
 # player.facing as (dx, dy) by the facing index of the player record (objects.py:33-34: left, right, up, down)
 FACING = ((-1, 0), (1, 0), (0, -1), (0, 1))
@@ -83,6 +90,30 @@ def check_levels(levels, mask, num_envs):
   if lo < -1 or hi > MAX_LEVEL:
     raise ValueError(f'levels must be -1 or world seeds in [0, {MAX_LEVEL}]')
   return arr, mask
+
+
+def pack_worlds(materials, creatures, area):
+  """Env.author_levels' worlds: materials (k, W, H) ids 1..12 and creatures (k, W, H) 0..3 (None: none), integer
+  tensors or arrays, as the uint8 (k, W * H) bytes of cr_author_levels (x-major, material | creature << 4), on the
+  device `materials` came on.  ValueError for a non-integer dtype or a wrong shape; a value out of range becomes
+  the byte 0xC0, which cr_author_levels rejects with status bit 1."""
+  def as_tensor(values, name):
+    if not torch.is_tensor(values):
+      values = np.asarray(values)
+      if values.dtype.kind not in 'iu':
+        raise ValueError(f'{name} must be integers, not {values.dtype}')
+      values = torch.from_numpy(values.astype(np.int64))
+    elif values.dtype.is_floating_point or values.dtype.is_complex or values.dtype == torch.bool:
+      raise ValueError(f'{name} must be integers, not {values.dtype}')
+    if values.dim() != 3 or tuple(values.shape[1:]) != tuple(area):
+      raise ValueError(f'{name} must have shape (k, {area[0]}, {area[1]}), not {tuple(values.shape)}')
+    return values.to(torch.int64)
+  mat = as_tensor(materials, 'materials')
+  cre = torch.zeros_like(mat) if creatures is None else as_tensor(creatures, 'creatures').to(mat.device)
+  if cre.shape != mat.shape:
+    raise ValueError(f'creatures must have the shape of materials, {tuple(mat.shape)}, not {tuple(cre.shape)}')
+  ok = (mat >= 1) & (mat <= 12) & (cre >= 0) & (cre <= 3)
+  return torch.where(ok, mat | (cre << 4), 0xC0).to(torch.uint8).reshape(mat.shape[0], -1)
 
 
 def _int_vector(values, name):
@@ -222,7 +253,8 @@ class Env:
   and its actions: set_levels / reset(levels=...) choose the world seeds (fixed evaluation worlds, finite
   training sets, level-replay curricula, replaying a logged episode); set_level_table / sample_levels make envs
   draw the world of every new episode from a weighted table of world seeds inside the step, and
-  set_level_weights updates the weights without a host read.  Returned tensors are views of the
+  set_level_weights updates the weights without a host read; author_levels puts caller-made worlds into table
+  entries and pin_levels puts envs on one entry.  Returned tensors are views of the
   env's output buffers: they are overwritten by the next `step()` / `reset()`; clone to keep them.
 
   Streams (the contract: include/crafter_b200.h, "Streams and ordering"): every call is ordered behind the work
@@ -489,7 +521,8 @@ class Env:
   @property
   def levels(self):
     """A copy of the current level of every env, int32 (num_envs,) (-1: the reference's sequence, -2 =
-    LEVEL_SAMPLED: drawn from the level table, see sample_levels)."""
+    LEVEL_SAMPLED: drawn from the level table, see sample_levels; LEVEL_PINNED_BASE - e = -3 - e: pinned to table
+    entry e, see pin_levels)."""
     return self._state['level'].clone()
 
   # ---- the level sampler ------------------------------------------------------------------------
@@ -633,6 +666,112 @@ class Env:
     per_world = sum(c[k].element_size() * c[k][0].numel() for k in ('mat', 'ents', 'meta', 'tag'))
     return dict(rows=rows, bytes_per_world=per_world,
                 bytes=per_world * rows + c['row'].element_size() * c['row'].numel())
+
+  # ---- authored levels and pinning ----------------------------------------------------------------
+  def _entries(self, entries, name, count=None):
+    """`entries` as int64 (k,) on the host-checked range [0, n) of the level table (one read)."""
+    if self._table is None:
+      raise RuntimeError(f'{name}: no level table (call set_level_table first)')
+    arr = _int_vector(entries, 'entries')
+    if count is not None and arr.numel() != count:
+      raise ValueError(f'entries must have shape ({count},), not {tuple(arr.shape)}')
+    return arr
+
+  def _check_entries(self, arr):
+    n = self._table_len
+    if arr.numel():
+      lo, hi = torch.stack([arr.min(), arr.max()]).tolist()
+      if lo < 0 or hi >= n:
+        raise ValueError(f'entries must be level table entries in [0, {n})')
+
+  def author_levels(self, entries, materials, creatures=None):
+    """Write caller-made worlds into the level table's entries (semantics: include/crafter_b200.h,
+    cr_author_levels): materials (k, W, H) ids 1..12 (the info['semantic'] ids), creatures (k, W, H) 0 none,
+    1 cow, 2 zombie, 3 skeleton (None: none), for the k entries of `entries` in [0, n).  An episode on an
+    authored entry i plays that world with every later draw keyed by seeds[i] and reports seeds[i] as its
+    world seed; the player starts at (W/2, H/2) as in every episode, so that cell must be grass, sand or path
+    without a creature, and creatures may stand on grass, sand and path only.  Sampled envs draw the entry
+    with its weight, and pin_levels plays it in every episode.
+
+    Turns the level cache on if it is off (the worlds live in its rows).  All or nothing: when any world is
+    rejected, ValueError names the worlds and the reasons and no entry changes.  Reads a status word per world
+    back, one synchronisation: this is the rare call.  An authored entry stays authored while its seed stays;
+    set_level_table with another seed for it generates that seed's world over it.  Reaches the envs that
+    already drew or were pinned to the entry from their second new episode at the latest; pin_levels or
+    sample_levels again makes it hold from the next."""
+    arr = self._entries(entries, 'author_levels')
+    worlds = pack_worlds(materials, creatures, self._area)
+    if worlds.shape[0] != arr.numel():
+      raise ValueError(f'{arr.numel()} entries for {worlds.shape[0]} worlds')
+    self._check_entries(arr)
+    with torch.cuda.device(self._device):
+      if self._cache is None:
+        self._fill_level_cache()
+      k = arr.numel()
+      if k == 0:
+        return
+      ent = arr.to(self._device, torch.int32)
+      worlds = worlds.to(self._device)
+      status = torch.empty(k, dtype=torch.int32, device=self._device)
+      s = self._enter()
+      _cabi.check(self._lib.cr_author_levels(self._handle, ent.data_ptr(), worlds.data_ptr(), k, status.data_ptr(), s))
+      self._exit()
+      status = status.cpu().numpy()
+    bad = np.flatnonzero(status)
+    if len(bad):
+      lines = [f'world {i} (entry {int(arr[i])}): ' + '; '.join(why for bit, why in AUTHOR_REASONS if status[i] & bit)
+               for i in bad[:8]]
+      more = f' (and {len(bad) - 8} more)' if len(bad) > 8 else ''
+      raise ValueError(f'author_levels: {len(bad)} of {k} worlds rejected, nothing changed{more}:\n' + '\n'.join(lines))
+
+  def level_worlds(self, entries):
+    """The worlds the level cache holds for `entries` (k,) in [0, n), decoded from its rows: {'materials': uint8
+    (k, W, H), 'creatures': uint8 (k, W, H) in author_levels' encoding, 'authored': bool (k,)}.  The read side of
+    an edit loop: read, change in torch, author_levels.  A generated row shows its world as generation left it,
+    so authoring it again under the same seed plays the same episodes."""
+    if self._cache is None:
+      raise RuntimeError('level_worlds: no level cache (call set_level_cache or author_levels first)')
+    arr = self._entries(entries, 'level_worlds')
+    self._check_entries(arr)
+    W, H = self._area
+    with torch.cuda.device(self._device):
+      idx = arr.to(self._device)
+      c, k = self._cache, arr.numel()
+      materials = (c['mat'][idx] & 0x0F).reshape(k, W, H)
+      ents = c['ents'][idx]
+      n = c['meta'][idx, 0].to(torch.int64)
+      kind = ents & 0xFF
+      slot = torch.arange(self._capacity, device=self._device)
+      live = (slot >= 2) & (slot < n[:, None]) & (kind >= 2) & (kind <= 4)
+      x, y = (ents >> 16) & 0xFFFF, (ents >> 32) & 0xFFFF
+      creatures = torch.zeros(k, W * H, dtype=torch.uint8, device=self._device)
+      world = torch.arange(k, device=self._device)[:, None].expand_as(ents)
+      creatures[world[live], (x * H + y)[live]] = (kind - 1)[live].to(torch.uint8)
+      authored = (c['meta'][idx, 1] & 4) != 0
+    return dict(materials=materials.contiguous(), creatures=creatures.reshape(k, W, H), authored=authored)
+
+  def pin_levels(self, entries, mask=None):
+    """Pin each env where `mask` is True (None: all) to level table entry entries[env] in [0, n): every new
+    episode of it plays that entry -- its seed, and its cached world (generated or authored) when the cache
+    holds it -- whatever the weights, so an entry of weight 0 can serve as an evaluation level that sampled envs
+    never draw.  `levels` shows LEVEL_PINNED_BASE - e.  Like set_levels it leaves the running episodes alone and
+    builds the next world of those envs once, now; reset(mask) right after it starts them at once.  Checked on
+    the host (ValueError; one read of device entries)."""
+    arr = self._entries(entries, 'pin_levels', self._num_envs)
+    with torch.cuda.device(self._device):
+      if mask is not None:
+        mask = torch.as_tensor(mask, device=self._device).to(torch.bool)
+        if tuple(mask.shape) != (self._num_envs,):
+          raise ValueError(f'mask must have shape ({self._num_envs},), not {tuple(mask.shape)}')
+      arr = arr.to(self._device)
+      self._check_entries(arr if mask is None else arr[mask])
+      self._level_in.copy_(arr if mask is None else torch.where(mask, arr, 0))
+      if mask is not None:
+        self._level_mask.copy_(mask)
+      s = self._enter()
+      _cabi.check(self._lib.cr_pin_levels(self._handle, None if mask is None else self._level_mask.data_ptr(),
+                                          self._level_in.data_ptr(), s))
+      self._exit()
 
   # ---- Env.step (env.py:83-118) ---------------------------------------------------------------
   def step(self, actions):

@@ -24,9 +24,10 @@ class ShardedEnv:
   """`crafter_b200.Env` over the whole job: `num_envs` is the GLOBAL batch; this process steps its
   own shard on `cuda:LOCAL_RANK`.  reset()/step() return the local shard's tensors.  Keyword arguments go to
   the env unchanged (e.g. `observation='semantic'` or `'symbolic'`: `gather` takes windows and float32 vectors
-  as it takes frames).  The env's other methods pass through: set_levels and sample_levels take the LOCAL
-  shard's levels and mask; set_level_table / set_level_weights take the same table on every rank, and since the
-  draw is keyed by the global env index the shards then play what one big batch plays."""
+  as it takes frames).  The env's other methods pass through: set_levels, sample_levels and pin_levels take the
+  LOCAL shard's levels, entries and mask; set_level_table / set_level_weights take the same table on every rank,
+  and author_levels the same worlds on every rank, and since the draw is keyed by the global env index the shards
+  then play what one big batch plays."""
 
   def __init__(self, num_envs, seed=0, env_factory=None, **kwargs):
     self.rank = dist.get_rank() if dist.is_initialized() else int(os.environ.get('RANK', 0))

@@ -154,6 +154,18 @@ class VectorEnv(_Base):
     """Env.set_level_cache: keep the level table's worlds generated on the device (memory for time)."""
     self.env.set_level_cache(enabled)
 
+  def author_levels(self, entries, materials, creatures=None):
+    """Env.author_levels: caller-made worlds into level table entries."""
+    self.env.author_levels(entries, materials, creatures)
+
+  def level_worlds(self, entries):
+    """Env.level_worlds: the worlds the level cache holds for these entries."""
+    return self.env.level_worlds(entries)
+
+  def pin_levels(self, entries, mask=None):
+    """Env.pin_levels: these envs play one level table entry in every new episode."""
+    self.env.pin_levels(entries, mask)
+
   def step(self, actions):
     obs, reward, done, info = self.env.step(actions)
     dead = self.env.state['final_stats'][:, 23] != 0

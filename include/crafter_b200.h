@@ -6,7 +6,7 @@
  * buffers are owned by the caller (torch tensors on the Python side) and passed as raw device
  * pointers; the library allocates no device memory (it owns a few auxiliary CUDA streams and events
  * per handle for the branches of the step graph, one 4-byte word for cr_error_flags and the scratch of
- * cr_fill_level_cache), starts no threads and is stream-ordered.
+ * cr_fill_level_cache and cr_author_levels), starts no threads and is stream-ordered.
  * Every function returns 0 on success and a negative code on error; cr_last_error() describes the
  * last failure of the calling thread.  A handle is bound to the device that was current in cr_create and is not re-entrant;
  * every entry point switches to that device for the duration of the call when another is current.
@@ -261,7 +261,8 @@ int cr_sample_levels(cr_handle *h, const uint8_t *mask, void *stream);
  *     row was never filled, the table or the cache was replaced after the draw -- generates the world as before.
  *     So a run with a cache is bit-identical to the same run without one, in every output and in all of cr_state
  *     (the permutation table `perm` is still computed for every world); only time and memory differ.
- *   - Envs on level -1 or on a fixed level generate their worlds as without a cache.
+ *   - Envs pinned to an entry (cr_pin_levels) note their entry like sampled envs and copy its row under the same
+ *     rule.  Envs on level -1 or on a fixed level generate their worlds as without a cache.
  *
  * cr_set_level_cache registers (or, with mat == NULL, removes) the cache: caller-owned DEVICE buffers, valid until
  * replaced, removed or cr_destroy:
@@ -272,8 +273,8 @@ int cr_sample_levels(cr_handle *h, const uint8_t *mask, void *stream);
  *   row   int32[num_envs][2]               scratch of k_seed: the entry each env's world of an episode parity was
  *                                          drawn from (any initial contents are harmless: only a tag match counts)
  * No stream: like cr_set_level_table it changes pointers only (the cached step graphs are captured again at the
- * next step).  Rows are filled by cr_fill_level_cache and by nothing else; a caller may write tags itself (-1
- * empties a row).
+ * next step).  Rows are written by cr_fill_level_cache and cr_author_levels and by nothing else; a caller may
+ * write tags itself (-1 empties a row).
  *
  * cr_fill_level_cache generates, on `stream`, the worlds of seeds[first, first + count) of the registered table
  * into their rows and tags them, skipping the rows already tagged with their entry's seed (entries at or beyond
@@ -283,6 +284,57 @@ int cr_sample_levels(cr_handle *h, const uint8_t *mask, void *stream);
  * slot_capacity + 12 bytes, 6,156 at the default geometry (64 x 64, slot_capacity 256). */
 int cr_set_level_cache(cr_handle *h, uint8_t *mat, void *ents, int32_t *meta, int32_t *tag, int32_t *row, int cap);
 int cr_fill_level_cache(cr_handle *h, int first, int count, void *stream);
+
+/* Authored levels: table entries whose cache row holds a world the caller made instead of the generated world of
+ * their seed, and envs pinned to one table entry.
+ *
+ * An entry i is authored when its cache row holds a caller-made world.  Everything else about the episode is what
+ * it is for the generated world of seeds[i]: every draw after the world is built (creature updates, balance, night
+ * noise) is keyed by seeds[i], PS_WORLD_SEED and final_world_seed report seeds[i], and the player starts at
+ * (W/2, H/2) with the reference's fresh vitals and inventory.  So an authored episode is a function of (authored
+ * world, seeds[i], actions) and replays bit for bit from those three.  The copy rule of the cache does not change:
+ * a row is installed when its tag equals the drawn seed.  cr_author_levels tags a row with seeds[i] as the table
+ * holds it when the row is written, so an authored row survives cr_fill_level_cache while its entry keeps that
+ * seed; once the caller rewrites seeds[i], the next fill generates the new seed's world over it (the cache's
+ * staleness rule).  meta[row][1] bit 2 (value 4) marks an authored row; it never reaches an env's state.
+ *
+ * cr_author_levels writes `count` worlds into the rows of entries[0, count), on `stream`:
+ *   entries  DEVICE int32[count]
+ *   worlds   DEVICE uint8[count][area_w * area_h], x-major (cell x * area_h + y, like cr_semantic); per byte:
+ *            bits 0-3 the material id 1..12 (info['semantic'] ids), bits 4-5 the creature (0 none, 1 cow,
+ *            2 zombie, 3 skeleton), bits 6-7 zero
+ *   status   DEVICE int32[count], written for every world: 0 = accepted, else the sum of
+ *              1  a byte out of range (material 0 or above 12, or bit 6 or 7 set)
+ *              2  a creature on a cell that is not grass, sand or path
+ *              4  the start cell (W/2, H/2) is not grass, sand or path, or holds a creature
+ *              8  more than slot_capacity - 2 creatures
+ *             16  the entry lies outside [0, min(table capacity, cache capacity)), or appears twice in the call
+ * All or nothing: when any world has a non-zero status, no row changes.  Otherwise each row gets the terrain
+ * (byte & 15); its creatures in slots 2 .. n - 1 in x-major cell order, with the records generation gives them
+ * (the step's own creature pass builds them); meta = {n, 1 | 4}; and last its tag, seeds[entry].  The table's *n
+ * is not looked at.  It touches no env state.  Its scratch is library-owned: 4 * (2 + 9 * cap) bytes for the
+ * smaller of the two capacities, allocated or grown by the call and freed by cr_destroy.  Fails without a table or
+ * a cache.
+ *
+ * Pinning: cr_pin_levels puts the envs whose mask byte is non-zero (mask == NULL: all) on table entry entries[env]
+ * (DEVICE int32[num_envs]); cr_state.level shows CR_LEVEL_PINNED(e).  Every new episode of a pinned env plays entry
+ * e: its world seed is seeds[e], read when the seed is decided, and its world is copied from row e of the cache
+ * when the row's tag is seeds[e] (an authored world, or a filled one), else generated.  The weights are not looked
+ * at: an entry of weight 0 is never sampled but can be pinned, so an evaluation suite can sit in the training
+ * table without being trained on.  A seed decided for an entry at or beyond *n (or a negative entry, or without a
+ * table) is the reference sequence's, and the env's sticky error bit 2 (value 4) is raised, as for an empty table.
+ * As in cr_set_levels, running episodes are left alone, and the prefetched next world and the seeds of the pinned
+ * envs are dropped and generated once on `stream`.  cr_set_levels or cr_sample_levels takes an env off its entry.
+ * Fails without a level table or when cr_state.level is NULL.
+ *
+ * Staleness, as for the weights: a world is read from its row when an env's next world is built, which happens in
+ * the step that starts the env's previous episode.  So a re-authored entry reaches an env that had already drawn or
+ * pinned it from its second new episode at the latest; calling cr_pin_levels / cr_sample_levels again for those
+ * envs makes it hold from the very next episode. */
+#define CR_LEVEL_PINNED(e) (-3 - (e))
+int cr_author_levels(cr_handle *h, const int32_t *entries, const uint8_t *worlds, int count, int32_t *status,
+                     void *stream);
+int cr_pin_levels(cr_handle *h, const uint8_t *mask, const int32_t *entries, void *stream);
 
 /* After the caller has written `mat` itself (state restore, tests): recount what the library keeps
  * incrementally about the terrain (the per-chunk counts of chunk_cnt; a no-op without that buffer
