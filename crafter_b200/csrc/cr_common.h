@@ -275,7 +275,14 @@ struct State {
   int32_t *lc_tag;          // [lc_cap] the world seed the row holds (a negative value: none)
   int32_t *lc_row;          // [B][2] table entry the world of each episode parity was drawn from, -1: none (k_seed)
   int32_t lc_cap;
+  // per-level episode statistics (cr_set_level_stats; caller-owned), not part of the ABI's cr_state
+  int32_t *lv_entry;        // [B][4] table entry episode e was decided from, at e & 3 (k_seed; -1: none), or null
+  int32_t *lv_final;        // [B] or null: the entry of the episode that ended last (the tick)
+  int64_t *lv_stats;        // [lv_cap][LV_COUNT] or null: what the tick adds per finished episode, LV_*
+  int32_t lv_cap;
 };
+// columns of a level statistics row (include/crafter_b200.h, cr_set_level_stats)
+constexpr int LV_EPISODES = 0, LV_DEAD = 1, LV_LENGTH = 2, LV_RETURN = 3, LV_RETURN_SQ = 4, LV_ACH = 5, LV_COUNT = 27;
 
 CR_DEV uint8_t *next_mat_of(const State &st, const Geom &g, int env) { return st.next_mat + (size_t)env * g.NC; }
 CR_DEV Ent *next_ents_of(const State &st, const Geom &g, int env) { return st.next_ents + (size_t)env * g.CAP; }
@@ -293,6 +300,7 @@ CR_DEV int cr_smem_fetch_add(uint16_t *p, int v) { int o = *p; *p = (uint16_t)(o
 CR_DEV int cr_atomic_inc(int32_t *p) { return (*p)++; }
 CR_DEV void cr_smem_or(uint32_t *p, uint32_t v) { *p |= v; }
 CR_DEV void cr_global_add(int32_t *p, int v) { *p += v; }
+CR_DEV void cr_global_add64(int64_t *p, int64_t v) { *p += v; }
 CR_DEV uint32_t cr_shfl(uint32_t v, int) { return v; }
 CR_DEV uint32_t cr_shfl_up(uint32_t v, int) { return v; }
 CR_DEV uint32_t cr_reduce_or(uint32_t v) { return v; }
@@ -316,6 +324,13 @@ CR_DEV int cr_smem_fetch_add(uint16_t *p, int v) {  // same, returning the old 1
 CR_DEV int cr_atomic_inc(int32_t *p) { return atomicAdd(p, 1); }
 CR_DEV void cr_smem_or(uint32_t *p, uint32_t v) { atomicOr(p, v); }
 CR_DEV void cr_global_add(int32_t *p, int v) { atomicAdd(p, v); }
+#ifdef CR_SIMT  // tests/simt runs every thread on one OS thread, where its atomics are plain read-modify-writes too
+CR_DEV void cr_global_add64(int64_t *p, int64_t v) { *p += v; }
+#else
+CR_DEV void cr_global_add64(int64_t *p, int64_t v) {  // two's complement: an unsigned add is the signed add
+  atomicAdd(reinterpret_cast<unsigned long long *>(p), (unsigned long long)v);
+}
+#endif
 CR_DEV uint32_t cr_shfl(uint32_t v, int src) { return __shfl_sync(0xffffffffu, v, src); }
 CR_DEV uint32_t cr_shfl_up(uint32_t v, int delta) { return __shfl_up_sync(0xffffffffu, v, delta); }
 CR_DEV uint32_t cr_reduce_or(uint32_t v) { return __reduce_or_sync(0xffffffffu, v); }

@@ -83,6 +83,7 @@ inline void state_from_abi(const cr_state &s, State &st) {
   st.lt_seeds = nullptr; st.lt_cum = nullptr; st.lt_n = nullptr; st.lt_cap = 0;  // cr_set_level_table
   st.lc_mat = nullptr; st.lc_ents = nullptr; st.lc_meta = nullptr; st.lc_tag = nullptr; st.lc_row = nullptr;
   st.lc_cap = 0;  // cr_set_level_cache
+  st.lv_entry = nullptr; st.lv_final = nullptr; st.lv_stats = nullptr; st.lv_cap = 0;  // cr_set_level_stats
 }
 
 }  // namespace cr

@@ -789,6 +789,25 @@ CR_DEV void env_balance(const Geom &g, const State &st, const double *daylight_t
 // balances (only the terminal frame can tell; the state is discarded).
 enum TickKind : int { TICK_FINAL = 0, TICK_BALANCE = 1, TICK_RESET = 2 };
 constexpr int FS_LENGTH = 22, FS_DEAD = 23, FS_INV = 24, FS_POS = 40, FS_COUNT = 42;  // final_stats row
+
+// A finished episode into the statistics row of the level table entry it was decided from (cr_set_level_stats).
+// Integer adds only, so the totals do not depend on the order of the envs or on how a batch is sharded.  `total`:
+// the episode's return, a sum of multiples of 0.1, so llrint(10 * total) is exact.
+CR_DEV void level_stats_count(const State &st, int env, const PlayerS *P, int length, bool dead, double total) {
+  const int32_t r = st.lv_entry[(size_t)env * 4 + (P->ps[PS_EPISODE] & 3)];
+  if (st.lv_final) st.lv_final[env] = r;
+  if (!st.lv_stats || r < 0 || r >= st.lv_cap) return;
+  int64_t *row = st.lv_stats + (size_t)r * LV_COUNT;
+  const int64_t tenths = llrint(10.0 * total);
+  cr_global_add64(row + LV_EPISODES, 1);
+  if (dead) cr_global_add64(row + LV_DEAD, 1);
+  cr_global_add64(row + LV_LENGTH, length);
+  cr_global_add64(row + LV_RETURN, tenths);
+  cr_global_add64(row + LV_RETURN_SQ, tenths * tenths);
+  for (int i = 0; i < N_ACH; ++i)
+    if (P->ach[i] > 0) cr_global_add64(row + LV_ACH + i, 1);
+}
+
 CR_DEV int env_step(const Geom &g, const State &st, const double *daylight_table, int env, int lane,
                      int action, PlayerS *P, Ent *sents, uint32_t *stouched, float *reward_out,
                      uint8_t *done_out, int auto_reset, int debug_skip = 0) {
@@ -889,6 +908,7 @@ CR_DEV int env_step(const Geom &g, const State &st, const double *daylight_table
       for (int i = 0; i < N_ITEMS; ++i) fs[FS_INV + i] = P->inv[i];
       fs[FS_POS] = P->ps[PS_PX]; fs[FS_POS + 1] = P->ps[PS_PY];
       if (st.final_world_seed) st.final_world_seed[env] = P->ps[PS_WORLD_SEED];  // before k_install replaces it
+      if (st.lv_entry) level_stats_count(st, env, P, step, dead, total);
       P->ps[PS_EP_LENGTH] = step;
       if (auto_reset) kind |= TICK_RESET;
     }

@@ -155,6 +155,9 @@ CR_DEV void wg_seed(const Geom &g, const State &st, int env, int lane, SeedScrat
     // the level cache row that may hold this world, by episode parity like perm (-1: none); only a hint, the
     // world is copied only if the row's tag is ws when it is built (wg_cached_row)
     if (st.lc_row) st.lc_row[(size_t)env * 2 + (episode & 1)] = (int32_t)entry;
+    // the entry the episode is counted under when it ends (cr_set_level_stats); four slots, since the seeds of the
+    // next two episodes are decided while this one runs
+    if (st.lv_entry) st.lv_entry[(size_t)env * 4 + (episode & 3)] = (int32_t)entry;
   }
   wg_perm(ws, perm, lane, S);  // only lane 0 uses `ws`
   if (ahead && lane == 0) nm[NM_AHEAD_VALID] = 1;

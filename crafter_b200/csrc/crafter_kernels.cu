@@ -624,6 +624,19 @@ int cr_set_level_cache(cr_handle *h, uint8_t *mat, void *ents, int32_t *meta, in
   return 0;
 }
 
+int cr_set_level_stats(cr_handle *h, int32_t *entry, int32_t *final_entry, int64_t *stats, int cap) {
+  if (!h) return fail_msg("null handle");
+  if (entry && stats && cap < 1) return fail_msg("cr_set_level_stats: stats without a capacity >= 1");
+  DeviceGuard on_device(h->device);
+  h->st.lv_entry = entry;
+  h->st.lv_final = entry ? final_entry : nullptr;
+  h->st.lv_stats = entry ? stats : nullptr;
+  h->st.lv_cap = entry && stats ? cap : 0;
+  for (GraphSlot &gs : h->slots)  // (as cr_set_level_table: the graphs hold a copy of `st`)
+    if (gs.exec) { cudaGraphExecDestroy(gs.exec); gs.exec = nullptr; }
+  return 0;
+}
+
 int cr_fill_level_cache(cr_handle *h, int first, int count, void *stream) {
   if (!h) return fail_msg("null handle");
   if (!h->st.lt_seeds) return fail_msg("cr_fill_level_cache: the handle has no level table (cr_set_level_table)");

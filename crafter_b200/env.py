@@ -29,6 +29,9 @@ AUTHOR_REASONS = ((1, 'a byte out of range (material outside 1..12 or creature o
                   (8, 'more than slot_capacity - 2 creatures'),
                   (16, 'the entry lies outside the cache, or appears twice in the call'))
 MAX_WEIGHT_TOTAL = 2 ** 32 - 1  # the largest total weight of a level table
+# the columns of a level statistics row (include/crafter_b200.h, cr_set_level_stats); 5.. are the achievements
+LEVEL_STATS = ('episodes', 'terminated', 'length', 'return_tenths', 'return_tenths_sq')
+LEVEL_STATS_COLUMNS = len(LEVEL_STATS) + len(rules.ACHIEVEMENTS)
 # player.facing as (dx, dy) by the facing index of the player record (objects.py:33-34: left, right, up, down)
 FACING = ((-1, 0), (1, 0), (0, -1), (0, 1))
 # The 22 channels of every window cell of observation='symbolic' (layout: include/crafter_b200.h,
@@ -164,6 +167,16 @@ def check_level_table(seeds, weights=None):
   return arr, w
 
 
+def level_scores(stats):
+  """(percent float64 (n, 22), score float64 (n,)) of Env.level_stats() rows, on their device: the success rate of
+  every achievement in percent of the entry's episodes (rules.ACHIEVEMENTS order) and the Crafter score, the
+  geometric mean with an offset of 1%, exp(mean(log(1 + percent))) - 1, as the reference's analysis computes them
+  (analysis/common.py:36, 47-55).  NaN for entries without episodes."""
+  episodes = stats['episodes'].to(torch.float64)
+  percent = 100 * stats['achievements'].to(torch.float64) / episodes[:, None]  # 0 / 0 = NaN
+  return percent, torch.exp(torch.log(1 + percent).mean(1)) - 1
+
+
 class Info(dict):
   """`info` of Env.step (env.py:108-115) as batched tensors; expensive entries are computed on
   first access: 'semantic' (engine.py:251-264), 'discount' (env.py:111) and -- for auto_reset, where
@@ -173,6 +186,9 @@ class Info(dict):
   'world_seed' int32 (B,): the world seed the current episode of each env plays; 'final_world_seed' int32 (B,):
   the world seed of the episode that ended in this step (rows with done=False hold older values or zeros) --
   with auto_reset, what Env.reset(levels=...) needs to replay that episode (see Env.set_levels).
+  With a level table: 'level_entry' int32 (B,), the table entry the current episode of each env was drawn from or
+  pinned to (-1: none); 'final_level_entry' int32 (B,), the entry of the episode that ended in this step (rows with
+  done=False hold older values or -1) -- what a learner-side level score is attributed by (see Env.level_stats).
 
   What the frame shows beyond the semantic ids (a semantic window shows every player as id 13):
   'facing' int32 (B, 2), the player's facing (dx, dy); 'sleeping' bool (B,); 'daylight' float32 (B,), the
@@ -213,6 +229,14 @@ class Info(dict):
       value = env._state['pstate'][:, state_lib.PS['world_seed']]
     elif key == 'final_world_seed':
       value = env._state['final_world_seed']
+    elif key in ('level_entry', 'final_level_entry'):
+      if env._ring is None:
+        raise KeyError(f'{key} needs a level table (Env.set_level_table)')
+      if key == 'final_level_entry':
+        value = env._ring['final']
+      else:
+        episode = env._state['pstate'][:, state_lib.PS['episode']].long() & 3
+        value = env._ring['entry'].gather(1, episode[:, None])[:, 0]
     elif key == 'local_semantic':
       value = env._local if env._observation == 'semantic' else env.local_semantic()
     else:
@@ -254,7 +278,8 @@ class Env:
   training sets, level-replay curricula, replaying a logged episode); set_level_table / sample_levels make envs
   draw the world of every new episode from a weighted table of world seeds inside the step, and
   set_level_weights updates the weights without a host read; author_levels puts caller-made worlds into table
-  entries and pin_levels puts envs on one entry.  Returned tensors are views of the
+  entries and pin_levels puts envs on one entry; set_level_stats / level_stats count every finished episode
+  against the entry it was drawn from, for the caller's level scores.  Returned tensors are views of the
   env's output buffers: they are overwritten by the next `step()` / `reset()`; clone to keep them.
 
   Streams (the contract: include/crafter_b200.h, "Streams and ordering"): every call is ordered behind the work
@@ -312,6 +337,8 @@ class Env:
     self._aux_handles = {}
     self._table, self._table_len = None, 0  # set_level_table
     self._cache = None  # set_level_cache
+    self._ring = None  # the entry notes of cr_set_level_stats, registered with the level table
+    self._stats = None  # set_level_stats
     self._needs_reset = True
     # raw addresses of the fixed buffers: the per-step calls below hand them to the C ABI without
     # touching torch again (the library switches to its own device itself, see DeviceGuard)
@@ -552,6 +579,8 @@ class Env:
       self._write_weights(weights.to(self._device), n)
       if self._cache is not None:  # new rows for a grown table; only the rows whose seed changed are generated
         self._fill_level_cache()
+      if self._ring is None or (self._stats is not None and self._stats.shape[0] < self._table['seeds'].numel()):
+        self._register_level_stats(self._stats is not None)
 
   def _write_weights(self, weights, n):
     """int64 device weights (n,) -> the kept copy and the inclusive cumulative sum as uint32 bit patterns."""
@@ -666,6 +695,78 @@ class Env:
     per_world = sum(c[k].element_size() * c[k][0].numel() for k in ('mat', 'ents', 'meta', 'tag'))
     return dict(rows=rows, bytes_per_world=per_world,
                 bytes=per_world * rows + c['row'].element_size() * c['row'].numel())
+
+  # ---- per-level episode statistics ------------------------------------------------------------------
+  def _register_level_stats(self, with_stats):
+    """Register the entry notes (allocated once, sized by the batch: filled with -1) and, with_stats, one statistics
+    row per row of the table's buffers, grown with the table (the rows counted so far are kept)."""
+    B = self._num_envs
+    if self._ring is None:
+      self._ring = dict(entry=torch.full((B, 4), -1, dtype=torch.int32, device=self._device),
+                        final=torch.full((B,), -1, dtype=torch.int32, device=self._device))
+      for v in self._ring.values():  # written by the env's stream: not reused by torch before that stream is done
+        v.record_stream(self._stream)
+    stats, rows = None, 0
+    if with_stats:
+      rows = self._table['seeds'].numel()
+      stats = self._stats
+      if stats is None or stats.shape[0] < rows:
+        stats = torch.zeros(rows, LEVEL_STATS_COLUMNS, dtype=torch.int64, device=self._device)
+        if self._stats is not None:  # (the last step ran on the env's stream, which _exit() made this stream wait for)
+          stats[:self._stats.shape[0]].copy_(self._stats)
+        stats.record_stream(self._stream)
+    _cabi.check(self._lib.cr_set_level_stats(self._handle, self._ring['entry'].data_ptr(), self._ring['final'].data_ptr(),
+                                             None if stats is None else stats.data_ptr(), rows))
+    self._stats = stats
+
+  def set_level_stats(self, enabled=True):
+    """Count every finished episode against the level table entry it was drawn from or pinned to (semantics:
+    include/crafter_b200.h, cr_set_level_stats): per entry, the episodes, the terminated ones, the summed length,
+    the summed return and its square in tenths (exact integers), and per achievement the episodes that unlocked it.
+    The step only adds integers, so the counts are exact, reproducible and the same however the batch is sharded;
+    level_stats() reads them and level_scores() or any torch code turns them into weights for set_level_weights,
+    without a host read.
+
+    enabled=True allocates one row per row of the table's buffers (216 bytes each), zeroed; the rows grow with the
+    table and keep their counts.  enabled=False frees them.  An episode counts when it ends while the statistics
+    are on; its entry was noted when its seed was decided, so an env moved off the table mid-episode still counts
+    that episode under the entry it was drawn from.  A done report counts once per step that reports it: without
+    auto_reset, stepping a done env again counts it again.  reset() of a running episode counts nothing.  Level -1
+    and fixed-level episodes are not counted."""
+    if not enabled:
+      if self._stats is not None:
+        self._register_level_stats(False)
+      return
+    if self._table is None:
+      raise RuntimeError('set_level_stats: no level table (call set_level_table first)')
+    with torch.cuda.device(self._device):
+      if self._stats is None:
+        self._register_level_stats(True)
+
+  def level_stats(self):
+    """Copies of the statistics rows of the n entries in use, made on the caller's stream (no host read):
+    {'episodes', 'terminated', 'length', 'return_tenths', 'return_tenths_sq': int64 (n,), 'achievements': int64
+    (n, 22) in rules.ACHIEVEMENTS order}.  The mean return of entry i is return_tenths[i] / (10 * episodes[i])."""
+    if self._stats is None:
+      raise RuntimeError('level_stats: the level statistics are off (call set_level_stats first)')
+    with torch.cuda.device(self._device):
+      rows = self._stats[:self._table_len]
+      out = {k: rows[:, i].clone(memory_format=torch.contiguous_format) for i, k in enumerate(LEVEL_STATS)}
+      out['achievements'] = rows[:, len(LEVEL_STATS):].clone(memory_format=torch.contiguous_format)
+    return out
+
+  def clear_level_stats(self, entries=None):
+    """Zero the statistics rows of `entries` in [0, n) (None: all), ordered on the caller's stream like every call:
+    how a caller keeps a window of recent episodes.  Checked on the host (ValueError; one read of device entries)."""
+    if self._stats is None:
+      raise RuntimeError('clear_level_stats: the level statistics are off (call set_level_stats first)')
+    with torch.cuda.device(self._device):
+      if entries is None:
+        self._stats.zero_()
+        return
+      arr = self._entries(entries, 'clear_level_stats')
+      self._check_entries(arr)
+      self._stats[arr.to(self._device)] = 0
 
   # ---- authored levels and pinning ----------------------------------------------------------------
   def _entries(self, entries, name, count=None):
@@ -924,9 +1025,17 @@ class Env:
     return state_lib.canonical(g('mat'), g('ents'), g('inventory'), g('achievements'), g('pstate'),
                                g('touched'), self._area)
 
-  def state_dict(self):
+  def state_dict(self, level_entries=False):
+    """Copies of the state tensors.  level_entries=True (with a level table) adds 'level_entry', the entry notes of
+    the running and the next two episodes (num_envs, 4), and 'final_level_entry', so that a restored batch counts
+    its running episodes under the entries they were drawn from (set_level_stats).  They are opt-in so that
+    snapshots of batches with and without a level table keep the same keys.  The level table, cache and statistics
+    are not env state."""
     torch.cuda.synchronize(self._device)
-    return {k: v.clone() for k, v in self._state.items()}
+    sd = {k: v.clone() for k, v in self._state.items()}
+    if level_entries and self._ring is not None:
+      sd['level_entry'], sd['final_level_entry'] = self._ring['entry'].clone(), self._ring['final'].clone()
+    return sd
 
   def load_state_dict(self, sd):
     # snapshots taken before levels existed: every env on the reference's sequence
@@ -934,11 +1043,20 @@ class Env:
     if 'level' not in sd and 'final_world_seed' not in sd:
       sd['level'] = torch.full_like(self._state['level'], -1)
       sd['final_world_seed'] = torch.zeros_like(self._state['final_world_seed'])
+    ring = {k: sd.pop(key) for k, key in (('entry', 'level_entry'), ('final', 'final_level_entry')) if key in sd}
     if set(sd) != set(self._state):
       raise ValueError(f'state_dict of another layout (keys differ: {sorted(set(sd) ^ set(self._state))})')
     torch.cuda.synchronize(self._device)
     for k, v in self._state.items():
       v.copy_(sd[k])
+    if ring and self._ring is None:
+      self._register_level_stats(False)
+    if self._ring is not None:  # snapshots without entry notes: no episode of theirs is attributed to an entry
+      for k, v in self._ring.items():
+        if k in ring:
+          v.copy_(ring[k])
+        else:
+          v.fill_(-1)
     self._needs_reset = False
 
   def recount(self):

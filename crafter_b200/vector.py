@@ -166,6 +166,18 @@ class VectorEnv(_Base):
     """Env.pin_levels: these envs play one level table entry in every new episode."""
     self.env.pin_levels(entries, mask)
 
+  def set_level_stats(self, enabled=True):
+    """Env.set_level_stats: count every finished episode against the level table entry it was drawn from."""
+    self.env.set_level_stats(enabled)
+
+  def level_stats(self):
+    """Env.level_stats: copies of the per-entry episode statistics."""
+    return self.env.level_stats()
+
+  def clear_level_stats(self, entries=None):
+    """Env.clear_level_stats: zero the statistics of these entries (None: all)."""
+    self.env.clear_level_stats(entries)
+
   def step(self, actions):
     obs, reward, done, info = self.env.step(actions)
     dead = self.env.state['final_stats'][:, 23] != 0

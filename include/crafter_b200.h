@@ -336,6 +336,40 @@ int cr_author_levels(cr_handle *h, const int32_t *entries, const uint8_t *worlds
                      void *stream);
 int cr_pin_levels(cr_handle *h, const uint8_t *mask, const int32_t *entries, void *stream);
 
+/* Per-level episode statistics: the step counts every finished episode against the level table entry it was drawn
+ * from, the signal a curriculum (prioritized level replay, ACCEL) computes its weights from.  The library only
+ * counts, in integers; scores and weights are the caller's.
+ *
+ * Entry notes: `entry` int32[num_envs][4] is a ring indexed by episode & 3.  Whenever the world seed of episode e of
+ * an env is decided, slot e & 3 gets the table entry it was drawn from (a sampled env) or pinned to (a pinned env), or
+ * -1 (level -1, a fixed level, an empty table, a pinned entry at or beyond *n).  Four slots, because while episode e
+ * runs the seeds of e + 1 (the prefetched world) and e + 2 (the ahead draw) are already decided.  cr_set_levels,
+ * cr_sample_levels and cr_pin_levels decide e + 1 and e + 2 again and note them again; the running episode keeps its
+ * note.  So an episode is counted under the entry it was drawn from, even when its env was moved off the table
+ * while it ran.
+ *
+ * Counting: for every env whose step reports done = 1, the tick reads r = entry[env][episode & 3], writes
+ * final_entry[env] = r (beside final_world_seed; rows of other envs are left alone) and, when 0 <= r < cap, adds to
+ * row r of `stats` int64[cap][27]:
+ *     0  1                                  episodes
+ *     1  1 if health <= 0                   terminated episodes (final_stats' dead flag)
+ *     2  the episode's length
+ *     3  llrint(10 * return)                the return in tenths, exact: every reward is a multiple of 0.1
+ *                                           (the return the env pays with reward=True, whatever cr_config.reward)
+ *     4  the square of column 3's addend
+ *     5 + i  1 if achievement i was unlocked (count >= 1) by the end (i in data.yaml order, 22 achievements)
+ * The adds are integer atomics: the totals are exact and do not depend on the order of threads or on how a batch is
+ * sharded over handles (sum the handles' rows).  A done report counts once per step that reports it: without
+ * auto_reset, stepping an env that is done again reports done again and counts again.  cr_reset of a running episode
+ * counts nothing.  Entries at or beyond `cap` are not counted.  An episode is counted when its seed was decided while
+ * the ring was registered and it ends while `stats` is registered.
+ *
+ * cr_set_level_stats registers caller-owned DEVICE buffers, valid until replaced, removed or cr_destroy: entry ==
+ * NULL removes all three; final_entry and stats are optional (NULL: not written; with a ring but no stats the notes
+ * are kept and nothing is counted).  The caller zeroes rows itself, stream-ordered, whenever it likes.  No stream:
+ * like cr_set_level_table it changes pointers only (the cached step graphs are captured again at the next step). */
+int cr_set_level_stats(cr_handle *h, int32_t *entry, int32_t *final_entry, int64_t *stats, int cap);
+
 /* After the caller has written `mat` itself (state restore, tests): recount what the library keeps
  * incrementally about the terrain (the per-chunk counts of chunk_cnt; a no-op without that buffer
  * or with CRAFTER_B200_INCR_CENSUS=0). */
