@@ -280,7 +280,13 @@ struct State {
   int32_t *lv_final;        // [B] or null: the entry of the episode that ended last (the tick)
   int64_t *lv_stats;        // [lv_cap][LV_COUNT] or null: what the tick adds per finished episode, LV_*
   int32_t lv_cap;
+  // level goals (cr_set_level_goals; caller-owned), not part of the ABI's cr_state
+  const int32_t *lg_goals;  // [lg_cap] achievement mask per table entry (bits 0..21; 0: the reference's reward), or null
+  int32_t *lg_notes;        // [B][4] the goal of episode e, at e & 3 (k_seed), read by the tick; null with lg_goals
+  int32_t lg_cap;
 };
+// the achievement bits of a level goal (bits 22..31 of a goals entry are ignored)
+constexpr uint32_t GOAL_BITS = (1u << 22) - 1;
 // columns of a level statistics row (include/crafter_b200.h, cr_set_level_stats)
 constexpr int LV_EPISODES = 0, LV_DEAD = 1, LV_LENGTH = 2, LV_RETURN = 3, LV_RETURN_SQ = 4, LV_ACH = 5, LV_COUNT = 27;
 

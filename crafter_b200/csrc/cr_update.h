@@ -880,6 +880,7 @@ CR_DEV int env_step(const Geom &g, const State &st, const double *daylight_table
   }
   if (lane == 0 && env < 4096) { cr_stamp(8192 + env, 3); cr_stamp(8192 + env, 5, traced_updates); cr_stamp(8192 + env, 6, n0); }
   int kind = TICK_FINAL;
+  uint32_t ended = 0;  // done, on lane 0
   uint32_t now = 0;  // achievements unlocked so far, one bit each (env.py:99-101), by all lanes
   for (int i = lane; i < N_ACH; i += CR_LANES) now |= (P->ach[i] > 0 ? 1u : 0u) << i;
   now = cr_reduce_or(now);
@@ -889,9 +890,19 @@ CR_DEV int env_step(const Geom &g, const State &st, const double *daylight_table
     P->ps[PS_LAST_HEALTH] = health;
     uint32_t unlocked = (uint32_t)P->ps[PS_UNLOCKED];
     if (now & ~unlocked) { P->ps[PS_UNLOCKED] = (int32_t)(unlocked | now); reward += 1.0; }
-    bool dead = health <= 0;
+    // final_stats' flag: 1 terminated (health <= 0, env.py:105-107), 2 the level goal reached
+    int term = health <= 0 ? 1 : 0;
+    // the running episode's level goal (cr_set_level_goals; 0: the reference's reward and ending).  Loaded here, not
+    // before the creature updates: held through them it cost k_update 4 to 6 registers
+    const uint32_t goal =
+        st.lg_notes ? (uint32_t)st.lg_notes[(size_t)env * 4 + (P->ps[PS_EPISODE] & 3)] & GOAL_BITS : 0u;
+    if (goal) {  // a level goal: 1 in the step that first reaches it and nothing else; reaching it ends the episode
+      const bool reached = ((unlocked | now) & goal) == goal;
+      reward = reached && (unlocked & goal) != goal ? 1.0 : 0.0;
+      term |= reached ? 2 : 0;
+    }
     bool over = g.length && step >= g.length;
-    bool done = dead || over;
+    bool done = term || over;
     reward_out[env] = (float)reward;  // info['reward']; the host zeroes it when reward=False
     done_out[env] = done ? 1 : 0;
     double *ret = st.ep_return + (size_t)env * 2;  // StatsRecorder bookkeeping, recorder.py:53-61
@@ -901,16 +912,16 @@ CR_DEV int env_step(const Geom &g, const State &st, const double *daylight_table
       ret[1] = total;
       // the terminal transition as the reference's info dict shows it (env.py:108-115); with
       // auto_reset the live rows already belong to the next episode when step() returns
+      // (achievements and inventory: by all lanes, below)
       int32_t *fs = st.final_stats + (size_t)env * FS_COUNT;
-      for (int i = 0; i < N_ACH; ++i) fs[i] = P->ach[i];
       fs[FS_LENGTH] = step;
-      fs[FS_DEAD] = dead ? 1 : 0;  // terminated (health <= 0) vs truncated (length reached), env.py:105-107
-      for (int i = 0; i < N_ITEMS; ++i) fs[FS_INV + i] = P->inv[i];
+      fs[FS_DEAD] = term;  // 0: truncated (length reached)
       fs[FS_POS] = P->ps[PS_PX]; fs[FS_POS + 1] = P->ps[PS_PY];
       if (st.final_world_seed) st.final_world_seed[env] = P->ps[PS_WORLD_SEED];  // before k_install replaces it
-      if (st.lv_entry) level_stats_count(st, env, P, step, dead, total);
+      if (st.lv_entry) level_stats_count(st, env, P, step, term & 1, total);
       P->ps[PS_EP_LENGTH] = step;
       if (auto_reset) kind |= TICK_RESET;
+      ended = 1;
     }
     // Spawn / despawn balancing (env.py:90-95) runs in env_balance right after this tick; it
     // touches neither health nor achievements, so reward / done above are already final.
@@ -922,6 +933,11 @@ CR_DEV int env_step(const Geom &g, const State &st, const double *daylight_table
                                       (kind == TICK_FINAL ? FRAME_FINAL : 0));
   }
   cr_syncwarp();
+  if (cr_shfl(ended, 0)) {  // the rest of the terminal record
+    int32_t *fs = st.final_stats + (size_t)env * FS_COUNT;
+    for (int i = lane; i < N_ACH; i += CR_LANES) fs[i] = P->ach[i];
+    for (int i = lane; i < N_ITEMS; i += CR_LANES) fs[FS_INV + i] = P->inv[i];
+  }
   for (int c = lane; c < g.TW; c += CR_LANES) E.touched[c] = stouched[c];
   for (int i = lane; i < N_ITEMS; i += CR_LANES) inv_g[i] = P->inv[i];
   for (int i = lane; i < N_ACH; i += CR_LANES) ach_g[i] = P->ach[i];

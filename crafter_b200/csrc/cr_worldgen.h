@@ -158,6 +158,11 @@ CR_DEV void wg_seed(const Geom &g, const State &st, int env, int lane, SeedScrat
     // the entry the episode is counted under when it ends (cr_set_level_stats); four slots, since the seeds of the
     // next two episodes are decided while this one runs
     if (st.lv_entry) st.lv_entry[(size_t)env * 4 + (episode & 3)] = (int32_t)entry;
+    // the episode's goal, fixed with its seed (cr_set_level_goals): the entry's mask, 0 without an entry below the
+    // goals' capacity (entry is ~0u without one)
+    if (st.lg_notes)
+      st.lg_notes[(size_t)env * 4 + (episode & 3)] =
+          entry < (uint32_t)st.lg_cap ? (int32_t)((uint32_t)wg_table_load(st.lg_goals + entry) & GOAL_BITS) : 0;
   }
   wg_perm(ws, perm, lane, S);  // only lane 0 uses `ws`
   if (ahead && lane == 0) nm[NM_AHEAD_VALID] = 1;

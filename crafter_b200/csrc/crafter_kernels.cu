@@ -637,6 +637,18 @@ int cr_set_level_stats(cr_handle *h, int32_t *entry, int32_t *final_entry, int64
   return 0;
 }
 
+int cr_set_level_goals(cr_handle *h, const int32_t *goals, int32_t *notes, int cap) {
+  if (!h) return fail_msg("null handle");
+  if (goals && (!notes || cap < 1)) return fail_msg("cr_set_level_goals: goals without notes or a capacity >= 1");
+  DeviceGuard on_device(h->device);
+  h->st.lg_goals = goals;
+  h->st.lg_notes = goals ? notes : nullptr;
+  h->st.lg_cap = goals ? cap : 0;
+  for (GraphSlot &gs : h->slots)  // (as cr_set_level_table: the graphs hold a copy of `st`)
+    if (gs.exec) { cudaGraphExecDestroy(gs.exec); gs.exec = nullptr; }
+  return 0;
+}
+
 int cr_fill_level_cache(cr_handle *h, int first, int count, void *stream) {
   if (!h) return fail_msg("null handle");
   if (!h->st.lt_seeds) return fail_msg("cr_fill_level_cache: the handle has no level table (cr_set_level_table)");

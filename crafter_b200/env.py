@@ -167,6 +167,24 @@ def check_level_table(seeds, weights=None):
   return arr, w
 
 
+def goal_mask(names):
+  """The level goal mask (Env.set_level_goals) of `names`: an achievement name, a sequence of names, or an int mask
+  over the 22 achievements (bit k = rules.ACHIEVEMENTS[k]).  ValueError for an unknown name or a bit above 21."""
+  if isinstance(names, str):
+    names = (names,)
+  if isinstance(names, (int, np.integer)) and not isinstance(names, (bool, np.bool_)):
+    mask = int(names)
+    if not 0 <= mask < 1 << len(rules.ACHIEVEMENTS):
+      raise ValueError(f'a goal mask must lie in [0, 2**{len(rules.ACHIEVEMENTS)}), not {mask}')
+    return mask
+  mask = 0
+  for name in names:
+    if not isinstance(name, str) or name not in rules.ACHIEVEMENTS:
+      raise ValueError(f'unknown achievement {name!r} (one of rules.ACHIEVEMENTS)')
+    mask |= 1 << rules.ACHIEVEMENTS.index(name)
+  return mask
+
+
 def level_scores(stats):
   """(percent float64 (n, 22), score float64 (n,)) of Env.level_stats() rows, on their device: the success rate of
   every achievement in percent of the entry's episodes (rules.ACHIEVEMENTS order) and the Crafter score, the
@@ -189,6 +207,9 @@ class Info(dict):
   With a level table: 'level_entry' int32 (B,), the table entry the current episode of each env was drawn from or
   pinned to (-1: none); 'final_level_entry' int32 (B,), the entry of the episode that ended in this step (rows with
   done=False hold older values or -1) -- what a learner-side level score is attributed by (see Env.level_stats).
+  'goal' int32 (B,): the level goal mask of the current episode of each env (0: the reference's reward; see
+  Env.set_level_goals); 'final_goal' int32 (B,): the goal of the episode that ended in this step, 0 in rows with
+  done=False.
 
   What the frame shows beyond the semantic ids (a semantic window shows every player as id 13):
   'facing' int32 (B, 2), the player's facing (dx, dy); 'sleeping' bool (B,); 'daylight' float32 (B,), the
@@ -205,7 +226,8 @@ class Info(dict):
       value = env.semantic()
     elif key == 'discount':
       # env.py:111: 1 - float(dead).  Taken from the terminal record of the tick (a regenerated env's
-      # inventory already shows the health of its next episode): dead is only ever set with done
+      # inventory already shows the health of its next episode): dead is only ever set with done.  Its flag is
+      # 1 * dead | 2 * reached (set_level_goals): a reached goal ends the task too, with discount 0
       dead = env._done & (env._state['final_stats'][:, 23] != 0)
       value = 1.0 - dead.float()
     elif key == 'final_achievements':
@@ -237,6 +259,16 @@ class Info(dict):
       else:
         episode = env._state['pstate'][:, state_lib.PS['episode']].long() & 3
         value = env._ring['entry'].gather(1, episode[:, None])[:, 0]
+    elif key in ('goal', 'final_goal'):
+      if env._goals is None:
+        value = torch.zeros(env.num_envs, dtype=torch.int32, device=env._device)
+      else:
+        episode = env._state['pstate'][:, state_lib.PS['episode']].long()
+        if key == 'final_goal':  # with auto_reset the episode that ended is the one before; its slot is still intact
+          episode = episode - int(env._auto_reset)
+        value = env._goals['notes'].gather(1, (episode & 3)[:, None])[:, 0]
+        if key == 'final_goal':
+          value = torch.where(env._done, value, 0)
     elif key == 'local_semantic':
       value = env._local if env._observation == 'semantic' else env.local_semantic()
     else:
@@ -279,7 +311,8 @@ class Env:
   draw the world of every new episode from a weighted table of world seeds inside the step, and
   set_level_weights updates the weights without a host read; author_levels puts caller-made worlds into table
   entries and pin_levels puts envs on one entry; set_level_stats / level_stats count every finished episode
-  against the entry it was drawn from, for the caller's level scores.  Returned tensors are views of the
+  against the entry it was drawn from, for the caller's level scores; set_level_goals gives entries achievement
+  goals that pay the reward and end the episode.  Returned tensors are views of the
   env's output buffers: they are overwritten by the next `step()` / `reset()`; clone to keep them.
 
   Streams (the contract: include/crafter_b200.h, "Streams and ordering"): every call is ordered behind the work
@@ -339,6 +372,7 @@ class Env:
     self._cache = None  # set_level_cache
     self._ring = None  # the entry notes of cr_set_level_stats, registered with the level table
     self._stats = None  # set_level_stats
+    self._goals = None  # set_level_goals: the goal table and the notes
     self._needs_reset = True
     # raw addresses of the fixed buffers: the per-step calls below hand them to the C ABI without
     # touching torch again (the library switches to its own device itself, see DeviceGuard)
@@ -581,6 +615,8 @@ class Env:
         self._fill_level_cache()
       if self._ring is None or (self._stats is not None and self._stats.shape[0] < self._table['seeds'].numel()):
         self._register_level_stats(self._stats is not None)
+      if self._goals is not None and self._goals['goals'].numel() < self._table['seeds'].numel():
+        self._register_level_goals()
 
   def _write_weights(self, weights, n):
     """int64 device weights (n,) -> the kept copy and the inclusive cumulative sum as uint32 bit patterns."""
@@ -767,6 +803,69 @@ class Env:
       arr = self._entries(entries, 'clear_level_stats')
       self._check_entries(arr)
       self._stats[arr.to(self._device)] = 0
+
+  # ---- level goals -----------------------------------------------------------------------------------
+  def _register_level_goals(self):
+    """Register the goal table, one entry per row of the table's buffers, grown with the table (the goals set so far
+    are kept, new entries are 0), and the notes (allocated once, sized by the batch: filled with 0)."""
+    rows = self._table['seeds'].numel()
+    old = self._goals
+    goals = torch.zeros(rows, dtype=torch.int32, device=self._device)
+    notes = torch.zeros(self._num_envs, 4, dtype=torch.int32, device=self._device) if old is None else old['notes']
+    if old is not None:  # (the last step ran on the env's stream, which _exit() made this stream wait for)
+      goals[:old['goals'].numel()].copy_(old['goals'])
+    for v in (goals, notes):  # read and written by the env's stream: not reused by torch before that stream is done
+      v.record_stream(self._stream)
+    _cabi.check(self._lib.cr_set_level_goals(self._handle, goals.data_ptr(), notes.data_ptr(), rows))
+    self._goals = dict(goals=goals, notes=notes)
+
+  def set_level_goals(self, goals):
+    """Give level table entries goals (semantics: include/crafter_b200.h, cr_set_level_goals): an episode drawn from
+    or pinned to entry i with goal G != 0 pays 1.0 in the step that first unlocks every achievement of G, and nothing
+    else (no health term), and that step ends it (done; final_stats' flag 2, so info['discount'] is 0 and
+    VectorEnv's `terminated` is True).  G = 0 is the reference's reward and ending.  So a (world, goal) pair is one
+    table entry, and sample_levels, set_level_weights, pin_levels, the level cache and level_stats work on tasks as
+    they do on worlds; a goal entry's successes are level_stats()['return_tenths'] / 10.
+
+    goals  (n,) ints, one achievement mask per table entry (bit k = rules.ACHIEVEMENTS[k]; see goal_mask), or a
+           list of n items that are each an achievement name, a sequence of names or an int; or None: no goals.
+    A device int tensor is only checked for dtype and shape and is not read back (nothing synchronises; bits 22..31
+    are ignored); host input is checked (ValueError for an unknown name or a bit above 21).
+
+    An episode's goal is fixed when its world seed is decided, so a rewritten goal has the staleness of rewritten
+    weights: it reaches an env from its third new episode at the latest, and from the next one after
+    sample_levels / pin_levels.  The goal table grows with the level table (new entries: 0).  Level -1 and
+    fixed-level episodes have no goal."""
+    if goals is None:
+      if self._goals is not None:
+        _cabi.check(self._lib.cr_set_level_goals(self._handle, None, None, 0))
+        self._goals = None
+      return
+    if self._table is None:
+      raise RuntimeError('set_level_goals: no level table (call set_level_table first)')
+    n = self._table_len
+    if torch.is_tensor(goals) and goals.is_cuda:
+      arr = _int_vector(goals, 'goals')
+    elif torch.is_tensor(goals) or isinstance(goals, np.ndarray):
+      arr = _int_vector(goals, 'goals')
+      bad = (arr < 0) | (arr >= 1 << len(rules.ACHIEVEMENTS))
+      if bool(bad.any()):
+        raise ValueError(f'goals must be masks in [0, 2**{len(rules.ACHIEVEMENTS)}) (entry {int(bad.nonzero()[0, 0])})')
+    else:
+      arr = torch.tensor([goal_mask(g) for g in goals], dtype=torch.int64)
+    if tuple(arr.shape) != (n,):
+      raise ValueError(f'goals must have shape ({n},), not {tuple(arr.shape)}')
+    with torch.cuda.device(self._device):
+      if self._goals is None:
+        self._register_level_goals()
+      self._goals['goals'][:n].copy_(arr.to(self._device))
+
+  @property
+  def level_goals(self):
+    """A copy of the goal masks of the n table entries in use, int32 (n,), or None without goals."""
+    if self._goals is None:
+      return None
+    return self._goals['goals'][:self._table_len].clone()
 
   # ---- authored levels and pinning ----------------------------------------------------------------
   def _entries(self, entries, name, count=None):
@@ -1030,11 +1129,14 @@ class Env:
     the running and the next two episodes (num_envs, 4), and 'final_level_entry', so that a restored batch counts
     its running episodes under the entries they were drawn from (set_level_stats).  They are opt-in so that
     snapshots of batches with and without a level table keep the same keys.  The level table, cache and statistics
-    are not env state."""
+    are not env state.  With level goals it adds 'level_goal', the goal notes (num_envs, 4), so that the running
+    episodes keep their goals; the goal table itself is not env state either."""
     torch.cuda.synchronize(self._device)
     sd = {k: v.clone() for k, v in self._state.items()}
     if level_entries and self._ring is not None:
       sd['level_entry'], sd['final_level_entry'] = self._ring['entry'].clone(), self._ring['final'].clone()
+    if level_entries and self._goals is not None:
+      sd['level_goal'] = self._goals['notes'].clone()
     return sd
 
   def load_state_dict(self, sd):
@@ -1044,6 +1146,7 @@ class Env:
       sd['level'] = torch.full_like(self._state['level'], -1)
       sd['final_world_seed'] = torch.zeros_like(self._state['final_world_seed'])
     ring = {k: sd.pop(key) for k, key in (('entry', 'level_entry'), ('final', 'final_level_entry')) if key in sd}
+    notes = sd.pop('level_goal', None)
     if set(sd) != set(self._state):
       raise ValueError(f'state_dict of another layout (keys differ: {sorted(set(sd) ^ set(self._state))})')
     torch.cuda.synchronize(self._device)
@@ -1057,6 +1160,13 @@ class Env:
           v.copy_(ring[k])
         else:
           v.fill_(-1)
+    if notes is not None and self._goals is None:  # goal notes into a batch without goals: a goal table of zeros
+      self.set_level_goals(torch.zeros(self._table_len, dtype=torch.int32, device=self._device))
+    if self._goals is not None:  # snapshots without goal notes: their running episodes have no goal
+      if notes is not None:
+        self._goals['notes'].copy_(notes)
+      else:
+        self._goals['notes'].fill_(0)
     self._needs_reset = False
 
   def recount(self):

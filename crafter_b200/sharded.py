@@ -28,7 +28,8 @@ class ShardedEnv:
   LOCAL shard's levels, entries and mask; set_level_table / set_level_weights take the same table on every rank,
   and author_levels the same worlds on every rank, and since the draw is keyed by the global env index the shards
   then play what one big batch plays.  level_stats gives the LOCAL shard's counts; they are integers, so their sum
-  over the ranks (an all-reduce) is exactly what one big batch counts."""
+  over the ranks (an all-reduce) is exactly what one big batch counts.  set_level_goals takes the same goals on
+every rank."""
 
   def __init__(self, num_envs, seed=0, env_factory=None, **kwargs):
     self.rank = dist.get_rank() if dist.is_initialized() else int(os.environ.get('RANK', 0))

@@ -13,8 +13,9 @@ the next episode), and the terminal transition travels in `info` under gymnasium
     info['final_obs'][i], info['final_info'][...][i]   valid where info['_final_obs'][i] (= done)
 
 (`final_observation` / `_final_observation` are kept as aliases for gymnasium <= 0.29 code.)
-`terminated` = the player died (`discount` 0 in the reference, env.py:105,111), `truncated` = the
-episode hit `length` (the registration's max_episode_steps).  `reset(options={'levels': levels})` (with or
+`terminated` = the player died (`discount` 0 in the reference, env.py:105,111) or reached its level goal
+(Env.set_level_goals: `discount` 0 too, success ends the task), `truncated` = the episode hit `length` (the
+registration's max_episode_steps).  `reset(options={'levels': levels})` (with or
 without 'reset_mask') and `set_levels(levels, mask)` choose the worlds the episodes play (Env.set_levels);
 `set_level_table`, `set_level_weights` and `sample_levels` make envs draw them from a weighted table inside the step
 (Env.set_level_table).  Arrays are torch.cuda tensors unless
@@ -177,6 +178,15 @@ class VectorEnv(_Base):
   def clear_level_stats(self, entries=None):
     """Env.clear_level_stats: zero the statistics of these entries (None: all)."""
     self.env.clear_level_stats(entries)
+
+  def set_level_goals(self, goals):
+    """Env.set_level_goals: achievement goals per level table entry that pay the reward and end the episode."""
+    self.env.set_level_goals(goals)
+
+  @property
+  def level_goals(self):
+    """Env.level_goals: a copy of the goal masks of the table entries in use, or None."""
+    return self.env.level_goals
 
   def step(self, actions):
     obs, reward, done, info = self.env.step(actions)

@@ -370,6 +370,38 @@ int cr_pin_levels(cr_handle *h, const uint8_t *mask, const int32_t *entries, voi
  * like cr_set_level_table it changes pointers only (the cached step graphs are captured again at the next step). */
 int cr_set_level_stats(cr_handle *h, int32_t *entry, int32_t *final_entry, int64_t *stats, int cap);
 
+/* Level goals: a level table entry can name the achievements its episodes must unlock.  Reaching them pays the
+ * reward and ends the episode, so a (world, goal) pair is one table entry, and the sampler, pinning, the cache and
+ * the statistics work on tasks as they work on worlds.
+ *
+ * Goal table: `goals` int32[cap]; entry i's goal G is a mask over the 22 achievements, bit k = achievement k in
+ * data.yaml order (the bit order of PS_UNLOCKED); bits 22..31 are ignored; G = 0 is the reference's reward and ending.
+ *
+ * When a goal is fixed: `notes` int32[num_envs][4] is a ring indexed by episode & 3, like the entry ring of
+ * cr_set_level_stats.  Whenever the world seed of episode e of an env is decided, slot e & 3 gets goals[r] (bits 0..21)
+ * for the entry r it was drawn from or pinned to, when r < cap; otherwise 0 (level -1, a fixed level, an empty table,
+ * a pinned entry at or beyond *n, an entry at or beyond the goals' capacity).  cr_set_levels, cr_sample_levels and
+ * cr_pin_levels decide e + 1 and e + 2 again and note them again; the running episode keeps its goal.  So a rewritten
+ * goal has the staleness of rewritten weights: it reaches an env from its third new episode at the latest, and from
+ * the next one after cr_sample_levels / cr_pin_levels.  An episode is a function of (world, seeds[i], G, actions).
+ * The notes do not need the statistics ring.
+ *
+ * What the tick does for an episode with G != 0, with `before` = PS_UNLOCKED before the step and `now` = the
+ * episode's unlocked mask after it; reached = (now & G) == G:
+ *   reward  1.0 in the step where (before & G) != G and the goal is reached, 0 in every other step: no health term,
+ *           other achievements pay nothing (cr_config.reward = 0 still zeroes the returned reward);
+ *   done    dead || over || reached: without auto_reset, stepping a reached env again reports done and pays 0;
+ *   final_stats[23]  1 * dead | 2 * reached (read as != 0 it is still "terminated": discount 0 on success);
+ *   ep_return and the statistics' return columns carry the paid reward (return_tenths = 10 * successes for a goal
+ *           entry); the statistics' terminated column keeps its meaning (health <= 0).
+ * PS_UNLOCKED, PS_LAST_HEALTH and the rest of the tick are unchanged.  For G = 0 nothing changes: a batch with goals
+ * registered, all 0, equals bit for bit the same batch without goals, in every output and in all of cr_state.
+ *
+ * cr_set_level_goals registers caller-owned DEVICE buffers, valid until replaced, removed or cr_destroy: goals ==
+ * NULL removes both.  The caller rewrites `goals` with stream-ordered writes whenever it likes.  No stream: like
+ * cr_set_level_stats it changes pointers only (the cached step graphs are captured again at the next step). */
+int cr_set_level_goals(cr_handle *h, const int32_t *goals, int32_t *notes, int cap);
+
 /* After the caller has written `mat` itself (state restore, tests): recount what the library keeps
  * incrementally about the terrain (the per-chunk counts of chunk_cnt; a no-op without that buffer
  * or with CRAFTER_B200_INCR_CENSUS=0). */
