@@ -11,6 +11,7 @@
 //                   the creatures in x-major cell order with the records generation gives them, and n
 //   k_author_tag    one thread per world: the row's meta (n, 1 | 4) and last its tag, when accepted; the claims are
 //                   released either way
+// cr_mutate_levels is k_mutate (below: the children of parent rows into the caller's worlds) and then these four.
 #pragma once
 #include "cr_kernels.h"
 
@@ -114,6 +115,107 @@ k_author_copy(Geom g, State st, const int32_t *__restrict__ entries, const uint8
     for (int k = tid; k < g.NC / 8; k += AUTHOR_THREADS) d8[k] = s8[k];
   } else {
     for (int c = tid; c < g.NC; c += AUTHOR_THREADS) dst[c] = src[c];
+  }
+}
+
+// cr_mutate_levels (include/crafter_b200.h): k_mutate writes the children into the caller's `worlds` in front of
+// the four launches above, which install them.  Its status bit comes beside AuthorStatus'.
+constexpr int MUTATE_PARENT = 32;  // the parent lies outside the capacity, or its row's tag is not seeds[parent]
+constexpr int MUTATE_OPS = 16;     // 0..11 set material o + 1, 12..14 place a cow / zombie / skeleton, 15 remove
+constexpr int MUTATE_CHUNK = AUTHOR_THREADS;  // edits drawn per round, one per thread
+struct MutateOps {
+  uint32_t cum[MUTATE_OPS];  // inclusive cumulative weights; cum[MUTATE_OPS - 1] is the total
+};
+
+// k_mutate: CTA i makes child i.  Thread 0 checks the parent row; the CTA copies its terrain (bits 0-3) into the
+// child's bytes and scatters the creatures of slots [2, n) into bits 4-5, counting them with a block sum.  Then, by
+// rounds of MUTATE_CHUNK edits, every thread draws one edit (cell and op) into shared memory and thread 0 applies
+// the round in order: edits are sequential by definition (one may undo, or make room for, the next).  A rejected
+// parent leaves a grass world behind, so its child's status names only the reasons that apply to it.  Parents are
+// only read: nothing writes a row before the launches behind this one.
+__global__ void __launch_bounds__(AUTHOR_THREADS)
+k_mutate(Geom g, State st, const int32_t *__restrict__ parents, const int32_t *__restrict__ children, int edits,
+         MutateOps ops, uint32_t key, int cap, uint8_t *__restrict__ worlds, int32_t *status, int32_t *scratch) {
+  __shared__ int s_ok, s_creatures;
+  __shared__ uint32_t s_cell[MUTATE_CHUNK];
+  __shared__ uint8_t s_op[MUTATE_CHUNK];
+  const int tid = threadIdx.x, i = blockIdx.x;
+  const int32_t p = parents[i];
+  if (tid == 0) {
+    const bool ok = p >= 0 && p < cap && st.lc_tag[p] == st.lt_seeds[p];
+    if (!ok) {
+      status[i] = MUTATE_PARENT;  // (zeroed before; this CTA is its only writer so far)
+      atomicOr(reinterpret_cast<unsigned *>(scratch), 1u);
+    }
+    s_ok = ok;
+    s_creatures = 0;
+  }
+  __syncthreads();
+  uint8_t *w = worlds + (size_t)i * g.NC;
+  const bool wide = (g.NC & 7) == 0 && (reinterpret_cast<uintptr_t>(worlds) & 7) == 0;  // rows stay 8-byte aligned
+  if (!s_ok) {
+    for (int c = tid; c < g.NC; c += AUTHOR_THREADS) w[c] = M_GRASS;
+    return;
+  }
+  const uint8_t *src = st.lc_mat + (size_t)p * g.NC;
+  if (wide) {
+    const uint64_t *s8 = reinterpret_cast<const uint64_t *>(src);
+    uint64_t *d8 = reinterpret_cast<uint64_t *>(w);
+    for (int k = tid; k < g.NC / 8; k += AUTHOR_THREADS) d8[k] = s8[k] & 0x0F0F0F0F0F0F0F0FULL;
+  } else {
+    for (int c = tid; c < g.NC; c += AUTHOR_THREADS) w[c] = src[c] & 0x0F;
+  }
+  __syncthreads();
+  const int n = st.lc_meta[(size_t)p * 2];
+  const Ent *ents = st.lc_ents + (size_t)p * g.CAP;
+  int count = 0;
+  for (int s = 2 + tid; s < n; s += AUTHOR_THREADS) {
+    const Ent e = ents[s];
+    if (e.type >= T_COW && e.type <= T_SKELETON) {
+      w[e.x * g.H + e.y] |= (uint8_t)((e.type - 1) << 4);
+      ++count;
+    }
+  }
+  if (count) atomicAdd(&s_creatures, count);
+  __syncthreads();  // the child's bytes and the count are complete, and visible to thread 0
+  int creatures = s_creatures;
+  const int start = (g.W / 2) * g.H + g.H / 2;
+  const uint32_t child = (uint32_t)children[i];
+  for (int base = 0; base < edits; base += MUTATE_CHUNK) {
+    const int j = base + tid;
+    if (j < edits) {
+      Rng r = rng_ctx(key, D_MUTATE, child);
+      r.k = 2u * (uint32_t)j;
+      const uint32_t c = rng_randint(r, (uint32_t)g.NC - 1u);
+      const uint32_t t = rng_randint(r, ops.cum[MUTATE_OPS - 1]);
+      int o = 0;  // the first o with t < cum[o]: the number of cum[k] <= t (cum is non-decreasing, t < total)
+#pragma unroll
+      for (int k = 0; k < MUTATE_OPS - 1; ++k) o += ops.cum[k] <= t;
+      s_cell[tid] = c + (c >= (uint32_t)start);
+      s_op[tid] = (uint8_t)o;
+    }
+    __syncthreads();
+    if (tid == 0) {
+      const int m = edits - base < MUTATE_CHUNK ? edits - base : MUTATE_CHUNK;
+      for (int k = 0; k < m; ++k) {
+        const int cell = (int)s_cell[k], o = s_op[k];
+        const int b = w[cell], mat = b & 0x0F, cre = b >> 4;
+        if (o < 12) {  // a material; a creature stays only on grass, sand or path
+          const bool keep = cre && author_walkable(o + 1);
+          creatures -= cre && !keep;
+          w[cell] = (uint8_t)((o + 1) | (keep ? cre << 4 : 0));
+        } else if (o < 15) {  // a creature of kind o - 11, on a walkable cell, within the slots
+          if (author_walkable(mat) && (cre || creatures < g.CAP - 2)) {
+            creatures += !cre;
+            w[cell] = (uint8_t)(mat | (o - 11) << 4);
+          }
+        } else if (cre) {  // remove the creature
+          --creatures;
+          w[cell] = (uint8_t)mat;
+        }
+      }
+    }
+    __syncthreads();  // the round's draws are applied before the next round overwrites them
   }
 }
 

@@ -111,7 +111,8 @@ struct alignas(8) Ent {
 
 // ---- keyed counter-based randomness (contract: oracle/keyed_rng.py) -------------------------
 enum Domain : uint32_t { D_SEED = 0, D_WG_MAT, D_WG_OBJ, D_UPDATE, D_BALANCE, D_NOISE,
-                         D_LEVEL };  // ctr (0,0,0,0), keyed by world_seed_of: the level table draw (wg_level_draw)
+                         D_LEVEL,    // ctr (0,0,0,0), keyed by world_seed_of: the level table draw (wg_level_draw)
+                         D_MUTATE };  // ctr (k, child entry, 0, 0), keyed by the caller's key: cr_mutate_levels' edits
 
 CR_DEV uint32_t mulhi32(uint32_t a, uint32_t b) {
 #ifdef CR_HOSTSIM

@@ -137,7 +137,7 @@ struct cr_handle {
   uint8_t *d2h_done;
   int32_t *err_word;  // cr_error_flags' reduction target
   FillScratch *fill;  // cr_fill_level_cache's scratch, allocated by its first call
-  int32_t *author;    // cr_author_levels' scratch (author_words(author_cap) int32), allocated and grown by it
+  int32_t *author;    // cr_author_levels' and cr_mutate_levels' scratch (author_words(author_cap) int32), grown by them
   int author_cap;
 };
 
@@ -510,6 +510,40 @@ int regenerate_relevelled(cr_handle *h, cudaStream_t s) {
   return 0;
 }
 
+// The entries' bound of cr_author_levels and cr_mutate_levels: the smaller of the table's and the cache's capacity.
+int author_cap_of(const cr_handle *h) { return h->st.lt_cap < h->st.lc_cap ? h->st.lt_cap : h->st.lc_cap; }
+
+// The scratch of cr_author_levels / cr_mutate_levels grown to `cap`, then its words and `status` zeroed on `s`.
+int author_begin(cr_handle *h, int cap, int32_t *status, int count, cudaStream_t s) {
+  if (h->author_cap < cap) {  // grown with the table and the cache, never shrunk; the claims start out free (-1)
+    if (h->author) CR_CUDA(cudaFree(h->author));
+    h->author = nullptr;
+    h->author_cap = 0;
+    CR_CUDA(cudaMalloc(&h->author, author_words(cap) * sizeof(int32_t)));
+    h->author_cap = cap;
+    CR_CUDA(cudaMemsetAsync(author_claim(h->author), 0xFF, (size_t)cap * sizeof(int32_t), s));
+  }
+  CR_CUDA(cudaMemsetAsync(h->author, 0, 2 * sizeof(int32_t), s));
+  CR_CUDA(cudaMemsetAsync(status, 0, (size_t)count * sizeof(int32_t), s));
+  return 0;
+}
+
+// The four launches that check `count` worlds and, unless any is rejected, install them into the rows of `entries`
+// (cr_author.h).  Returns the number of launches.
+int launch_author(cr_handle *h, const int32_t *entries, const uint8_t *worlds, int count, int cap, int32_t *status,
+                  cudaStream_t s) {
+  const Geom &g = h->g;
+  int32_t *scratch = h->author;
+  k_author_check<<<count, AUTHOR_THREADS, 0, s>>>(g, h->st, entries, worlds, cap, status, scratch);
+  k_author_copy<<<count, AUTHOR_THREADS, 0, s>>>(g, h->st, entries, worlds, count, scratch);
+  const State as = author_state(h->st, scratch, h->author_cap);
+  CR_LAUNCH(k_wg_obj, h->is_default, count < h->num_sms * 2 ? count : h->num_sms * 2, OBJ_THREADS, 0, s, g, as, entries,
+            scratch + 1, 0);
+  k_author_tag<<<(count + 255) / 256, 256, 0, s>>>(h->st, entries, count, cap, scratch, h->author_cap);
+  CR_CUDA(cudaGetLastError());
+  return 4;
+}
+
 }  // namespace
 
 // The handle's streams, events and graphs belong to the device that was current in cr_create;
@@ -690,27 +724,43 @@ int cr_author_levels(cr_handle *h, const int32_t *entries, const uint8_t *worlds
   if (!entries || !worlds || !status) return fail_msg("null argument");
   DeviceGuard on_device(h->device);
   cudaStream_t s = (cudaStream_t)stream;
-  const Geom &g = h->g;
-  const int cap = h->st.lt_cap < h->st.lc_cap ? h->st.lt_cap : h->st.lc_cap;
-  if (h->author_cap < cap) {  // grown with the table and the cache, never shrunk; the claims start out free (-1)
-    if (h->author) CR_CUDA(cudaFree(h->author));
-    h->author = nullptr;
-    h->author_cap = 0;
-    CR_CUDA(cudaMalloc(&h->author, author_words(cap) * sizeof(int32_t)));
-    h->author_cap = cap;
-    CR_CUDA(cudaMemsetAsync(author_claim(h->author), 0xFF, (size_t)cap * sizeof(int32_t), s));
+  const int cap = author_cap_of(h);
+  int k;
+  if ((k = author_begin(h, cap, status, count, s)) < 0) return k;
+  if ((k = launch_author(h, entries, worlds, count, cap, status, s)) < 0) return k;
+  h->launches += k;
+  return 0;
+}
+
+int cr_mutate_levels(cr_handle *h, const int32_t *parents, const int32_t *children, int count, int edits,
+                     const uint32_t *weights, uint32_t key, uint8_t *worlds, int32_t *status, void *stream) {
+  if (!h) return fail_msg("null handle");
+  if (!h->st.lt_seeds) return fail_msg("cr_mutate_levels: the handle has no level table (cr_set_level_table)");
+  if (!h->st.lc_mat) return fail_msg("cr_mutate_levels: the handle has no level cache (cr_set_level_cache)");
+  if (count < 0) return fail_msg("cr_mutate_levels: negative count");
+  if (edits < 0 || edits > CR_MUTATE_MAX_EDITS) return fail_msg("cr_mutate_levels: edits outside [0, CR_MUTATE_MAX_EDITS]");
+  MutateOps ops = {};
+  if (edits > 0) {  // the weights are read here, before the call returns
+    if (!weights) return fail_msg("null argument");
+    uint64_t total = 0;
+    for (int o = 0; o < MUTATE_OPS; ++o) {
+      total += weights[o];
+      ops.cum[o] = (uint32_t)total;
+    }
+    if (total == 0 || total > 0xFFFFFFFFull)
+      return fail_msg("cr_mutate_levels: the total of the weights lies outside [1, 2**32 - 1]");
   }
-  int32_t *scratch = h->author;
-  CR_CUDA(cudaMemsetAsync(scratch, 0, 2 * sizeof(int32_t), s));
-  CR_CUDA(cudaMemsetAsync(status, 0, (size_t)count * sizeof(int32_t), s));
-  k_author_check<<<count, AUTHOR_THREADS, 0, s>>>(g, h->st, entries, worlds, cap, status, scratch);
-  k_author_copy<<<count, AUTHOR_THREADS, 0, s>>>(g, h->st, entries, worlds, count, scratch);
-  const State as = author_state(h->st, scratch, h->author_cap);
-  CR_LAUNCH(k_wg_obj, h->is_default, count < h->num_sms * 2 ? count : h->num_sms * 2, OBJ_THREADS, 0, s, g, as, entries,
-            scratch + 1, 0);
-  k_author_tag<<<(count + 255) / 256, 256, 0, s>>>(h->st, entries, count, cap, scratch, h->author_cap);
-  CR_CUDA(cudaGetLastError());
-  h->launches += 4;
+  if (count == 0) return 0;
+  if (!parents || !children || !worlds || !status) return fail_msg("null argument");
+  DeviceGuard on_device(h->device);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int cap = author_cap_of(h);
+  int k;
+  if ((k = author_begin(h, cap, status, count, s)) < 0) return k;
+  k_mutate<<<count, AUTHOR_THREADS, 0, s>>>(h->g, h->st, parents, children, edits, ops, key, cap, worlds, status,
+                                            h->author);
+  if ((k = launch_author(h, children, worlds, count, cap, status, s)) < 0) return k;
+  h->launches += 1 + k;
   return 0;
 }
 

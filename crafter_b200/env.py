@@ -28,6 +28,12 @@ AUTHOR_REASONS = ((1, 'a byte out of range (material outside 1..12 or creature o
                   (4, 'the start cell (W/2, H/2) is not grass, sand or path, or holds a creature'),
                   (8, 'more than slot_capacity - 2 creatures'),
                   (16, 'the entry lies outside the cache, or appears twice in the call'))
+# cr_mutate_levels' status bit beyond AUTHOR_REASONS: why a child was rejected
+MUTATE_REASONS = AUTHOR_REASONS + (
+    (32, 'the parent lies outside the cache, or its row does not hold its current world'),)
+# cr_mutate_levels' edit kinds, in op order: set a material (rules.MATERIALS), place a creature, remove a creature
+MUTATE_OPS = tuple(rules.MATERIALS) + ('cow', 'zombie', 'skeleton', 'remove')
+MAX_MUTATE_EDITS = 4096  # CR_MUTATE_MAX_EDITS
 MAX_WEIGHT_TOTAL = 2 ** 32 - 1  # the largest total weight of a level table
 # the columns of a level statistics row (include/crafter_b200.h, cr_set_level_stats); 5.. are the achievements
 LEVEL_STATS = ('episodes', 'terminated', 'length', 'return_tenths', 'return_tenths_sq')
@@ -117,6 +123,28 @@ def pack_worlds(materials, creatures, area):
     raise ValueError(f'creatures must have the shape of materials, {tuple(mat.shape)}, not {tuple(cre.shape)}')
   ok = (mat >= 1) & (mat <= 12) & (cre >= 0) & (cre <= 3)
   return torch.where(ok, mat | (cre << 4), 0xC0).to(torch.uint8).reshape(mat.shape[0], -1)
+
+
+def mutate_weights(weights):
+  """Env.mutate_levels' weights as a list of MUTATE_OPS ints: None (every op 1), a sequence of 16 ints in op order,
+  or a dict {op name: weight} (missing ops: 0).  ValueError for an unknown name, a wrong length, a non-integer or
+  negative weight, or a total outside [1, MAX_WEIGHT_TOTAL]."""
+  if weights is None:
+    return [1] * len(MUTATE_OPS)
+  if isinstance(weights, dict):
+    unknown = set(weights) - set(MUTATE_OPS)
+    if unknown:
+      raise ValueError(f'unknown mutation ops {sorted(map(str, unknown))} (one of MUTATE_OPS)')
+    weights = [weights.get(name, 0) for name in MUTATE_OPS]
+  a = np.asarray(weights.cpu() if torch.is_tensor(weights) else weights)
+  if a.dtype.kind not in 'iu' or a.shape != (len(MUTATE_OPS),):
+    raise ValueError(f'weights must be {len(MUTATE_OPS)} integers (MUTATE_OPS order) or a dict, not {a.dtype} {a.shape}')
+  w = [int(v) for v in a]
+  if min(w) < 0:
+    raise ValueError('mutation weights must be non-negative')
+  if not 1 <= sum(w) <= MAX_WEIGHT_TOTAL:
+    raise ValueError(f'the total mutation weight must lie in [1, {MAX_WEIGHT_TOTAL}], not {sum(w)}')
+  return w
 
 
 def _int_vector(values, name):
@@ -949,6 +977,68 @@ class Env:
       creatures[world[live], (x * H + y)[live]] = (kind - 1)[live].to(torch.uint8)
       authored = (c['meta'][idx, 1] & 4) != 0
     return dict(materials=materials.contiguous(), creatures=creatures.reshape(k, W, H), authored=authored)
+
+  def mutate_levels(self, parents, children, edits, key, weights=None):
+    """Make children of level table entries on the device (semantics: include/crafter_b200.h, cr_mutate_levels):
+    child i starts as the world the cache holds for parents[i], takes `edits` keyed random edits and is authored
+    into entry children[i] (the mutator of ACCEL).  An edit sets a material, places a creature or removes one
+    (MUTATE_OPS); edits keep the world valid, so a child of a valid world is never rejected for its bytes.  A child
+    is a function of (parent world, key, child entry, edits, weights): the same call on every rank makes the same
+    children, and a caller varies `key` between calls.
+
+    parents, children  (k,) ints in [0, n); children distinct; a child may be its own parent or another's parent.
+    edits              int in [0, MAX_MUTATE_EDITS].
+    key                int in [0, 2**32).
+    weights            None (every op 1), 16 ints in MUTATE_OPS order, or a dict {op name: weight}.
+    Checked on the host (ValueError; one read of device entries).  Turns the level cache on if it is off.  A parent
+    whose row does not hold its entry's current world (a seed rewritten without a fill) is rejected.  All or nothing,
+    as author_levels: ValueError names the rejected children and the reasons, and no entry changes.  Reads a status
+    word per child back, one synchronisation.  The children's statistics and goals are left alone.
+
+    Returns {'materials': uint8 (k, W, H), 'creatures': uint8 (k, W, H)}: the children, as author_levels takes
+    them."""
+    arr_p = self._entries(parents, 'mutate_levels')
+    arr_c = self._entries(children, 'mutate_levels', arr_p.numel())
+    if isinstance(edits, bool) or not isinstance(edits, (int, np.integer)) or not 0 <= edits <= MAX_MUTATE_EDITS:
+      raise ValueError(f'edits must be an int in [0, {MAX_MUTATE_EDITS}], not {edits!r}')
+    if isinstance(key, bool) or not isinstance(key, (int, np.integer)) or not 0 <= key < 2 ** 32:
+      raise ValueError(f'key must be an int in [0, 2**32), not {key!r}')
+    w = mutate_weights(weights)
+    k, n = arr_p.numel(), self._table_len
+    if k:
+      both = torch.cat([arr_p, arr_c.to(arr_p.device)])
+      srt = torch.sort(arr_c).values
+      dup = (srt[1:] == srt[:-1]).any() if k > 1 else torch.zeros((), dtype=torch.bool)
+      lo, hi, twice = torch.stack([both.min(), both.max(), dup.to(both.device, torch.int64)]).tolist()  # one read
+      if lo < 0 or hi >= n:
+        raise ValueError(f'entries must be level table entries in [0, {n})')
+      if twice:
+        raise ValueError('children must be distinct')
+    W, H = self._area
+    with torch.cuda.device(self._device):
+      if self._cache is None:
+        self._fill_level_cache()
+      if k == 0:
+        empty = torch.zeros(0, W, H, dtype=torch.uint8, device=self._device)
+        return dict(materials=empty, creatures=empty.clone())
+      par = arr_p.to(self._device, torch.int32)
+      chi = arr_c.to(self._device, torch.int32)
+      worlds = torch.empty(k, W * H, dtype=torch.uint8, device=self._device)
+      status = torch.empty(k, dtype=torch.int32, device=self._device)
+      host_w = (ctypes.c_uint32 * len(MUTATE_OPS))(*w)
+      s = self._enter()
+      _cabi.check(self._lib.cr_mutate_levels(self._handle, par.data_ptr(), chi.data_ptr(), k, int(edits), host_w,
+                                             int(key), worlds.data_ptr(), status.data_ptr(), s))
+      self._exit()
+      status = status.cpu().numpy()
+    bad = np.flatnonzero(status)
+    if len(bad):
+      lines = [f'child {i} (entry {int(arr_c[i])}, parent {int(arr_p[i])}): ' +
+               '; '.join(why for bit, why in MUTATE_REASONS if status[i] & bit) for i in bad[:8]]
+      more = f' (and {len(bad) - 8} more)' if len(bad) > 8 else ''
+      raise ValueError(f'mutate_levels: {len(bad)} of {k} children rejected, nothing changed{more}:\n' + '\n'.join(lines))
+    worlds = worlds.reshape(k, W, H)
+    return dict(materials=worlds & 0x0F, creatures=worlds >> 4)
 
   def pin_levels(self, entries, mask=None):
     """Pin each env where `mask` is True (None: all) to level table entry entries[env] in [0, n): every new

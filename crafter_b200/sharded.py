@@ -27,7 +27,9 @@ class ShardedEnv:
   as it takes frames).  The env's other methods pass through: set_levels, sample_levels and pin_levels take the
   LOCAL shard's levels, entries and mask; set_level_table / set_level_weights take the same table on every rank,
   and author_levels the same worlds on every rank, and since the draw is keyed by the global env index the shards
-  then play what one big batch plays.  level_stats gives the LOCAL shard's counts; they are integers, so their sum
+  then play what one big batch plays.  mutate_levels makes the same children on every rank when every rank makes
+  the same call: a child is a function of its parent's world, the key, its entry, the edits and the weights alone,
+  so no bytes need to be broadcast.  level_stats gives the LOCAL shard's counts; they are integers, so their sum
   over the ranks (an all-reduce) is exactly what one big batch counts.  set_level_goals takes the same goals on
 every rank."""
 

@@ -163,6 +163,10 @@ class VectorEnv(_Base):
     """Env.level_worlds: the worlds the level cache holds for these entries."""
     return self.env.level_worlds(entries)
 
+  def mutate_levels(self, parents, children, edits, key, weights=None):
+    """Env.mutate_levels: children of level table entries, made by keyed random edits of their worlds."""
+    return self.env.mutate_levels(parents, children, edits, key, weights)
+
   def pin_levels(self, entries, mask=None):
     """Env.pin_levels: these envs play one level table entry in every new episode."""
     self.env.pin_levels(entries, mask)

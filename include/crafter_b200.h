@@ -24,7 +24,8 @@
  *     `stream` afterwards sees them, other streams must wait on it.  Output buffers are overwritten by the next
  *     call that writes them, in stream order: a reader on another stream must be waited on before that call.
  *   - Host memory: cr_step_host and cr_error_flags synchronise `stream` before they return, so their host
- *     buffers are read and written by then; no other entry point touches host memory.
+ *     buffers are read and written by then; cr_mutate_levels reads its host weights before it returns; no other
+ *     entry point touches host memory.
  *   - Several handles, on one device or several, may be used from one thread or from one thread each; a single
  *     handle is not re-entrant and must not be used from two threads at once.
  * Env (crafter_b200/env.py) keeps this contract on a private stream per env that waits on the caller's current
@@ -335,6 +336,45 @@ int cr_fill_level_cache(cr_handle *h, int first, int count, void *stream);
 int cr_author_levels(cr_handle *h, const int32_t *entries, const uint8_t *worlds, int count, int32_t *status,
                      void *stream);
 int cr_pin_levels(cr_handle *h, const uint8_t *mask, const int32_t *entries, void *stream);
+
+/* Level mutation: children of table entries made by keyed random edits of their worlds, on the device (the mutator
+ * of ACCEL-style curricula).  Every child is valid by construction, and a function of (parent world, key, child
+ * entry, edits, weights) alone: not of its position in the call, nor of the handle or the rank.
+ *
+ * cr_mutate_levels makes `count` children on `stream`; child i goes to entry children[i] and is made from the row of
+ * entry parents[i] (DEVICE int32[count] each):
+ *   Decode   child i starts as the world that row holds: materials are lc_mat & 15, creatures come from its slots
+ *            [2, n) whose type is cow, zombie or skeleton, in cr_author_levels' encoding (bits 4-5 = 1, 2, 3).
+ *            Generated and authored rows alike.
+ *   Edits    then `edits` edits, in order, each on the world the one before left.  Edit j of child i makes two draws
+ *            with key (key, 7) (7: the draw domain MUTATE) and counter (k, children[i], 0, 0), k = 2j and 2j + 1,
+ *            each w = word 0 of Philox4x32-10 and randint(m) = (w * m) >> 32:
+ *              c = randint(W*H - 1), cell = c + (c >= start), start = (W/2) * H + H/2: the start cell is never edited
+ *                  (cells x-major, x * H + y, as in the rows);
+ *              r = randint(T), T = the total of the weights; the op is the first o with r < cum[o] (cum: the
+ *                  inclusive cumulative weights).
+ *   Ops      0..11   set material o + 1 (data.yaml order); when it is not grass, sand or path, a creature on the
+ *                    cell is removed;
+ *            12..14  place a cow, zombie or skeleton: nothing on a cell that is not grass, sand or path; on a cell
+ *                    that holds a creature, its kind is replaced; otherwise nothing when the world already holds
+ *                    slot_capacity - 2 creatures;
+ *            15      remove the creature on the cell, if any.
+ *            So a child passes cr_author_levels' checks whenever its parent's world does.
+ *   weights  HOST uint32[CR_MUTATE_OPS], read before the call returns; may be NULL when edits == 0.
+ *   worlds   DEVICE uint8[count][area_w * area_h], caller-owned: the children, in cr_author_levels' encoding.
+ *   status   DEVICE int32[count], as cr_author_levels writes it, plus
+ *             32  the parent lies outside [0, min(table capacity, cache capacity)), or its row's tag is not
+ *                 seeds[parent] (the row does not hold that entry's current world).
+ * All parents are read before any row is written, so a child may be its own parent or the parent of another child of
+ * the same call.  The children are then installed by cr_author_levels' own launches: all or nothing (when any status
+ * word is non-zero no row changes, and the contents of `worlds` are unspecified); accepted rows are authored (meta
+ * bit 2) and tagged seeds[child]; the staleness is authoring's.  Five launches: the edit kernel, then authoring's four.
+ * Fails without a table or a cache, when edits lies outside [0, CR_MUTATE_MAX_EDITS], or when edits > 0 and the total
+ * of the weights lies outside [1, 2**32 - 1]. */
+#define CR_MUTATE_OPS 16
+#define CR_MUTATE_MAX_EDITS 4096
+int cr_mutate_levels(cr_handle *h, const int32_t *parents, const int32_t *children, int count, int edits,
+                     const uint32_t *weights, uint32_t key, uint8_t *worlds, int32_t *status, void *stream);
 
 /* Per-level episode statistics: the step counts every finished episode against the level table entry it was drawn
  * from, the signal a curriculum (prioritized level replay, ACCEL) computes its weights from.  The library only
