@@ -48,7 +48,7 @@ EXPORTS = ('cr_abi_version', 'cr_last_error', 'cr_create', 'cr_destroy', 'cr_res
            'cr_timing', 'cr_source_hash', 'cr_error_flags', 'cr_step_local', 'cr_local',
            'cr_step_symbolic', 'cr_symbolic', 'cr_set_levels', 'cr_set_level_table', 'cr_sample_levels',
            'cr_set_level_cache', 'cr_fill_level_cache', 'cr_author_levels', 'cr_pin_levels',
-           'cr_set_level_stats', 'cr_set_level_goals', 'cr_mutate_levels')
+           'cr_set_level_stats', 'cr_set_level_goals', 'cr_set_level_starts', 'cr_mutate_levels')
 
 _lib = None
 
@@ -83,6 +83,7 @@ def declare(lib, prefix='cr_'):
     lib.cr_mutate_levels.argtypes = [vp, vp, vp, ctypes.c_int, ctypes.c_int, vp, ctypes.c_uint32, vp, vp, vp]
     lib.cr_set_level_stats.argtypes = [vp, vp, vp, vp, ctypes.c_int]
     lib.cr_set_level_goals.argtypes = [vp, vp, vp, ctypes.c_int]
+    lib.cr_set_level_starts.argtypes = [vp, vp, vp, ctypes.c_int]
     lib.cr_launch_count.argtypes = [vp]
     lib.cr_launch_count.restype = ctypes.c_int64
     lib.cr_error_flags.argtypes = [vp, vp, vp]

@@ -87,6 +87,8 @@ enum ErrBits : int {
   ERR_DAYLIGHT_CLAMP = 2,  // the env's step ran past the daylight table: the last entry is used from there on
   ERR_LEVEL_TABLE = 4,     // a sampled env was seeded from an empty level table, or a pinned env from an entry at or
                            // beyond its *n: that episode plays world_seed_of
+  ERR_LEVEL_START = 8,     // an installed episode's level start was on but not applicable: it started at the
+                           // reference's start (cr_set_level_starts)
 };
 constexpr int32_t LEVEL_SAMPLED = -2;  // level[env]: every new episode draws its world from the level table (cr_sample_levels)
 constexpr int32_t LEVEL_PINNED_BASE = -3;  // level[env] = -3 - e: every new episode plays table entry e (cr_pin_levels)
@@ -285,9 +287,15 @@ struct State {
   const int32_t *lg_goals;  // [lg_cap] achievement mask per table entry (bits 0..21; 0: the reference's reward), or null
   int32_t *lg_notes;        // [B][4] the goal of episode e, at e & 3 (k_seed), read by the tick; null with lg_goals
   int32_t lg_cap;
+  // level starts (cr_set_level_starts; caller-owned), not part of the ABI's cr_state
+  const int32_t *ls_starts;  // [ls_cap][START_WORDS] the player's start per table entry (word 0: on), or null
+  int32_t *ls_notes;         // [B][4][START_WORDS] the start of episode e, at e & 3 (k_seed), read by k_install
+  int32_t ls_cap;
 };
 // the achievement bits of a level goal (bits 22..31 of a goals entry are ignored)
 constexpr uint32_t GOAL_BITS = (1u << 22) - 1;
+// words of a level start record (include/crafter_b200.h, cr_set_level_starts): on, x, y, facing, inventory[16]
+constexpr int START_ON = 0, START_X = 1, START_Y = 2, START_FACING = 3, START_INV = 4, START_WORDS = 20;
 // columns of a level statistics row (include/crafter_b200.h, cr_set_level_stats)
 constexpr int LV_EPISODES = 0, LV_DEAD = 1, LV_LENGTH = 2, LV_RETURN = 3, LV_RETURN_SQ = 4, LV_ACH = 5, LV_COUNT = 27;
 

@@ -85,6 +85,7 @@ inline void state_from_abi(const cr_state &s, State &st) {
   st.lc_cap = 0;  // cr_set_level_cache
   st.lv_entry = nullptr; st.lv_final = nullptr; st.lv_stats = nullptr; st.lv_cap = 0;  // cr_set_level_stats
   st.lg_goals = nullptr; st.lg_notes = nullptr; st.lg_cap = 0;  // cr_set_level_goals
+  st.ls_starts = nullptr; st.ls_notes = nullptr; st.ls_cap = 0;  // cr_set_level_starts
 }
 
 }  // namespace cr

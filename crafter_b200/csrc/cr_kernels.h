@@ -443,6 +443,10 @@ __global__ void __launch_bounds__(INSTALL_THREADS) k_install(Geom g, State st) {
   for (int r = blockIdx.x; r < count; r += gridDim.x) {
     const int env = st.reset_list[r];
     wg_install_scatter(g, st, env, threadIdx.x, INSTALL_THREADS);
+    // with level starts the player may stand off the centre, on a cell another thread is still scattering a creature
+    // to; without them the centre is known to be empty.  Keyed to the registration, not to the env's note, because
+    // only thread 0 reads which episode it installs (st is a kernel argument: uniform over the CTA)
+    if (st.ls_notes) __syncthreads();
     if (threadIdx.x == 0) wg_install_player(g, st, env);
     __syncthreads();
   }

@@ -164,6 +164,14 @@ CR_DEV void wg_seed(const Geom &g, const State &st, int env, int lane, SeedScrat
       st.lg_notes[(size_t)env * 4 + (episode & 3)] =
           entry < (uint32_t)st.lg_cap ? (int32_t)((uint32_t)wg_table_load(st.lg_goals + entry) & GOAL_BITS) : 0;
   }
+  // the episode's level start, fixed with its seed (cr_set_level_starts): the entry's record, zeros without an entry
+  // below the starts' capacity.  One word per lane, with lane 0's entry
+  if (st.ls_notes) {
+    const uint32_t e = cr_shfl(entry, 0);
+    int32_t *note = st.ls_notes + ((size_t)env * 4 + (episode & 3)) * START_WORDS;
+    for (int w = lane; w < START_WORDS; w += CR_LANES)
+      note[w] = e < (uint32_t)st.ls_cap ? wg_table_load(st.ls_starts + (size_t)e * START_WORDS + w) : 0;
+  }
   wg_perm(ws, perm, lane, S);  // only lane 0 uses `ws`
   if (ahead && lane == 0) nm[NM_AHEAD_VALID] = 1;
 }
@@ -497,37 +505,58 @@ CR_DEV void wg_install_scatter(const Geom &g, const State &st, int env, int tid,
   }
 }
 
-// Phase C (one thread): Player + per-episode scalars, env.py:75-79, objects.py:70-82,
-// data.yaml:39-55; consumes the prefetched world.
-// Player + per-episode scalars of a fresh episode, env.py:75-79, objects.py:70-82, data.yaml:39-55.
+// The level start of `episode` (cr_set_level_starts) when it is on and applicable, else null: a record that is on but
+// not applicable raises ERR_LEVEL_START and the episode starts at the reference's start.  After the creatures are
+// scattered: the start cell must be grass, sand or path and hold no creature.
+CR_DEV const int32_t *wg_level_start(const Geom &g, const State &st, int env, int episode) {
+  if (!st.ls_notes) return nullptr;
+  const int32_t *s = st.ls_notes + ((size_t)env * 4 + (episode & 3)) * START_WORDS;
+  if (!s[START_ON]) return nullptr;
+  const int x = s[START_X], y = s[START_Y], facing = s[START_FACING];
+  bool ok = x >= 0 && x < g.W && y >= 0 && y < g.H && facing >= 0 && facing < 4 && s[START_INV] >= 1;
+  for (int i = 0; i < N_ITEMS; ++i) ok = ok && s[START_INV + i] >= 0 && s[START_INV + i] <= 9;
+  if (ok) {
+    const size_t c = (size_t)env * g.NC + (size_t)x * g.H + y;
+    ok = ((WALKABLE >> (st.mat[c] & MAT_MASK)) & 1u) && st.objmap[c] == 0;
+  }
+  if (!ok) st.pstate[(size_t)env * PS_COUNT + PS_ERROR] |= ERR_LEVEL_START;
+  return ok ? s : nullptr;
+}
+
+// Phase C (one thread): Player + per-episode scalars of a fresh episode, env.py:75-79, objects.py:70-82,
+// data.yaml:39-55.  `start` (a level start record, or null): the player stands at its (x, y) with its facing and
+// inventory instead of at (W/2, H/2), facing down, with data.yaml's initial inventory.
 CR_DEV void wg_fresh_player(const Geom &g, const State &st, int env, int n_slots, int episode,
-                            int world_seed) {
+                            int world_seed, const int32_t *start = nullptr) {
   int32_t *ps = st.pstate + (size_t)env * PS_COUNT;
   int32_t *inv = st.inventory + (size_t)env * N_ITEMS;
   int32_t *ach = st.achievements + (size_t)env * N_ACH;
-  for (int i = 0; i < N_ITEMS; ++i) inv[i] = i < 4 ? 9 : 0;
+  const int px = start ? start[START_X] : g.W / 2, py = start ? start[START_Y] : g.H / 2;
+  const int health = start ? start[START_INV] : 9;
+  for (int i = 0; i < N_ITEMS; ++i) inv[i] = start ? start[START_INV + i] : i < 4 ? 9 : 0;
   for (int i = 0; i < N_ACH; ++i) ach[i] = 0;
   ps[PS_HUNGER2] = 0; ps[PS_THIRST2] = 0; ps[PS_FATIGUE] = 0; ps[PS_RECOVER2] = 0;
-  ps[PS_SLEEPING] = 0; ps[PS_P_LAST_HEALTH] = 9; ps[PS_LAST_HEALTH] = 9; ps[PS_UNLOCKED] = 0;
+  ps[PS_SLEEPING] = 0; ps[PS_P_LAST_HEALTH] = health; ps[PS_LAST_HEALTH] = health; ps[PS_UNLOCKED] = 0;
   ps[PS_NSLOTS] = n_slots; ps[PS_STEP] = 0;
   ps[PS_EPISODE] = episode; ps[PS_WORLD_SEED] = world_seed;
-  ps[PS_PX] = g.W / 2; ps[PS_PY] = g.H / 2;
+  ps[PS_PX] = px; ps[PS_PY] = py;
   st.ep_return[(size_t)env * 2] = 0.0;
   Ent p;
-  p.type = T_PLAYER; p.health = 9; p.x = (int16_t)(g.W / 2); p.y = (int16_t)(g.H / 2);
-  p.aux = 3;  // facing (0, 1) = down, objects.py:72
+  p.type = T_PLAYER; p.health = (int8_t)health; p.x = (int16_t)px; p.y = (int16_t)py;
+  p.aux = (int16_t)(start ? start[START_FACING] : 3);  // facing; 3: (0, 1) = down, objects.py:72
   Ent *ents = st.ents + (size_t)env * g.CAP;
   ents[1] = p;
   ents[0].type = T_NONE;
-  st.objmap[(size_t)env * g.NC + (g.W / 2) * g.H + g.H / 2] = 1;  // env.py:76-78
-  int ch = ((g.W / 2) / CHUNK) * g.ncy + ((g.H / 2) / CHUNK);
+  st.objmap[(size_t)env * g.NC + px * g.H + py] = 1;  // env.py:76-78
+  int ch = (px / CHUNK) * g.ncy + (py / CHUNK);
   cr_atomic_or(&st.touched[(size_t)env * g.TW + (ch >> 5)], 1u << (ch & 31));
 }
 
 // Phase C (one thread): consumes the prefetched world.
 CR_DEV void wg_install_player(const Geom &g, const State &st, int env) {
   int32_t *nm = st.next_meta + (size_t)env * NM_COUNT;
-  wg_fresh_player(g, st, env, nm[NM_NSLOTS], nm[NM_EPISODE], nm[NM_WORLD_SEED]);
+  wg_fresh_player(g, st, env, nm[NM_NSLOTS], nm[NM_EPISODE], nm[NM_WORLD_SEED],
+                  wg_level_start(g, st, env, nm[NM_EPISODE]));
   if (nm[NM_VALID] & 2) st.pstate[(size_t)env * PS_COUNT + PS_ERROR] |= ERR_SLOT_OVERFLOW;  // found by k_wg_obj
   nm[NM_VALID] = 0;
   // the seed prepared ahead (next to k_wg_obj) becomes the seed of the world to generate next

@@ -683,6 +683,20 @@ int cr_set_level_goals(cr_handle *h, const int32_t *goals, int32_t *notes, int c
   return 0;
 }
 
+static_assert(CR_START_WORDS == START_WORDS, "the start record of the header and of the kernels");
+
+int cr_set_level_starts(cr_handle *h, const int32_t *starts, int32_t *notes, int cap) {
+  if (!h) return fail_msg("null handle");
+  if (starts && (!notes || cap < 1)) return fail_msg("cr_set_level_starts: starts without notes or a capacity >= 1");
+  DeviceGuard on_device(h->device);
+  h->st.ls_starts = starts;
+  h->st.ls_notes = starts ? notes : nullptr;
+  h->st.ls_cap = starts ? cap : 0;
+  for (GraphSlot &gs : h->slots)  // (as cr_set_level_table: the graphs hold a copy of `st`)
+    if (gs.exec) { cudaGraphExecDestroy(gs.exec); gs.exec = nullptr; }
+  return 0;
+}
+
 int cr_fill_level_cache(cr_handle *h, int first, int count, void *stream) {
   if (!h) return fail_msg("null handle");
   if (!h->st.lt_seeds) return fail_msg("cr_fill_level_cache: the handle has no level table (cr_set_level_table)");

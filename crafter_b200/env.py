@@ -36,6 +36,9 @@ MUTATE_OPS = tuple(rules.MATERIALS) + ('cow', 'zombie', 'skeleton', 'remove')
 MAX_MUTATE_EDITS = 4096  # CR_MUTATE_MAX_EDITS
 MAX_WEIGHT_TOTAL = 2 ** 32 - 1  # the largest total weight of a level table
 # the columns of a level statistics row (include/crafter_b200.h, cr_set_level_stats); 5.. are the achievements
+START_WORDS = 20  # CR_START_WORDS: a level start record is on, x, y, facing, then the 16 items (Env.set_level_starts)
+FACING_NAMES = ('left', 'right', 'up', 'down')  # the facing index of a start record (FACING order)
+ERR_LEVEL_START = 8  # error_flags: a level start was on but not applicable; that episode started at the reference's
 LEVEL_STATS = ('episodes', 'terminated', 'length', 'return_tenths', 'return_tenths_sq')
 LEVEL_STATS_COLUMNS = len(LEVEL_STATS) + len(rules.ACHIEVEMENTS)
 # player.facing as (dx, dy) by the facing index of the player record (objects.py:33-34: left, right, up, down)
@@ -213,6 +216,59 @@ def goal_mask(names):
   return mask
 
 
+def level_start(inventory=None, pos=None, facing='down', area=(64, 64)):
+  """One level start record (Env.set_level_starts): int32 (20,) with `on` = 1.
+
+  inventory  {item name: amount} (rules.ITEMS); items it leaves out take the reference's initial values (data.yaml:
+             9 health, food, drink and energy, nothing else).  Every amount lies in [0, 9], health in [1, 9].
+  pos        (x, y) inside `area`, or None: the reference's start (W/2, H/2).
+  facing     'left', 'right', 'up', 'down', or a (dx, dy) pair of FACING.
+  ValueError for an unknown name, a value out of range or a position outside the area.  Whether the world's cell can
+  hold the player (grass, sand or path, no creature) is decided on the device, when the episode is installed."""
+  W, H = (int(v) for v in area)
+  row = np.zeros(START_WORDS, np.int32)
+  row[0] = 1
+  x, y = (W // 2, H // 2) if pos is None else pos
+  if not (isinstance(x, (int, np.integer)) and isinstance(y, (int, np.integer)) and 0 <= x < W and 0 <= y < H):
+    raise ValueError(f'a start position must be integers (x, y) inside the area {W} x {H}, not {pos!r}')
+  row[1:3] = x, y
+  if isinstance(facing, str):
+    if facing not in FACING_NAMES:
+      raise ValueError(f'unknown facing {facing!r} (one of {FACING_NAMES})')
+    row[3] = FACING_NAMES.index(facing)
+  else:
+    try:
+      row[3] = FACING.index(tuple(int(v) for v in facing))
+    except (TypeError, ValueError):
+      raise ValueError(f'a facing is a name of {FACING_NAMES} or a (dx, dy) of {FACING}, not {facing!r}') from None
+  inv = [rules.ITEM_INITIAL.get(name, 0) for name in rules.ITEMS]
+  for name, amount in (inventory or {}).items():
+    if name not in rules.ITEMS:
+      raise ValueError(f'unknown item {name!r} (one of rules.ITEMS)')
+    if not isinstance(amount, (int, np.integer)) or isinstance(amount, (bool, np.bool_)):
+      raise ValueError(f'the amount of {name} must be an int, not {amount!r}')
+    inv[rules.ITEMS.index(name)] = int(amount)
+  row[4:] = inv
+  _check_starts(row[None], area)
+  return row
+
+
+def _check_starts(rows, area):
+  """Start records (k, 20) int64 checked on the host: on in {0, 1}; the records that are on lie inside `area`, face
+  one of the four directions, and hold items in [0, 9] with health in [1, 9].  ValueError naming the first bad row."""
+  rows = np.asarray(rows, np.int64)
+  W, H = area
+  on = rows[:, 0] != 0
+  inv = rows[:, 4:]
+  bad = (rows[:, 0] < 0) | (rows[:, 0] > 1) | on & (
+      (rows[:, 1] < 0) | (rows[:, 1] >= W) | (rows[:, 2] < 0) | (rows[:, 2] >= H) | (rows[:, 3] < 0) |
+      (rows[:, 3] > 3) | (inv < 0).any(1) | (inv > rules.ITEM_MAX).any(1) | (inv[:, 0] < 1))
+  if bad.any():
+    i = int(np.flatnonzero(bad)[0])
+    raise ValueError(f'start {i} is not a level start record (on 0 or 1; x, y inside {W} x {H}; facing 0..3; items '
+                     f'in [0, 9], health in [1, 9]): {rows[i].tolist()}')
+
+
 def level_scores(stats):
   """(percent float64 (n, 22), score float64 (n,)) of Env.level_stats() rows, on their device: the success rate of
   every achievement in percent of the entry's episodes (rules.ACHIEVEMENTS order) and the Crafter score, the
@@ -340,7 +396,8 @@ class Env:
   set_level_weights updates the weights without a host read; author_levels puts caller-made worlds into table
   entries and pin_levels puts envs on one entry; set_level_stats / level_stats count every finished episode
   against the entry it was drawn from, for the caller's level scores; set_level_goals gives entries achievement
-  goals that pay the reward and end the episode.  Returned tensors are views of the
+  goals that pay the reward and end the episode, and set_level_starts the player's start position, facing,
+  inventory and vitals.  Returned tensors are views of the
   env's output buffers: they are overwritten by the next `step()` / `reset()`; clone to keep them.
 
   Streams (the contract: include/crafter_b200.h, "Streams and ordering"): every call is ordered behind the work
@@ -401,6 +458,7 @@ class Env:
     self._ring = None  # the entry notes of cr_set_level_stats, registered with the level table
     self._stats = None  # set_level_stats
     self._goals = None  # set_level_goals: the goal table and the notes
+    self._starts = None  # set_level_starts: the start table and the notes
     self._needs_reset = True
     # raw addresses of the fixed buffers: the per-step calls below hand them to the C ABI without
     # touching torch again (the library switches to its own device itself, see DeviceGuard)
@@ -645,6 +703,8 @@ class Env:
         self._register_level_stats(self._stats is not None)
       if self._goals is not None and self._goals['goals'].numel() < self._table['seeds'].numel():
         self._register_level_goals()
+      if self._starts is not None and self._starts['starts'].shape[0] < self._table['seeds'].numel():
+        self._register_level_starts()
 
   def _write_weights(self, weights, n):
     """int64 device weights (n,) -> the kept copy and the inclusive cumulative sum as uint32 bit patterns."""
@@ -894,6 +954,88 @@ class Env:
     if self._goals is None:
       return None
     return self._goals['goals'][:self._table_len].clone()
+
+  # ---- level starts ------------------------------------------------------------------------------------
+  def _register_level_starts(self):
+    """Register the start table, one record per row of the table's buffers, grown with the table (the starts set so
+    far are kept, new entries are 0), and the notes (allocated once, sized by the batch: filled with 0)."""
+    rows = self._table['seeds'].numel()
+    old = self._starts
+    starts = torch.zeros(rows, START_WORDS, dtype=torch.int32, device=self._device)
+    notes = (torch.zeros(self._num_envs, 4, START_WORDS, dtype=torch.int32, device=self._device)
+             if old is None else old['notes'])
+    if old is not None:  # (the last step ran on the env's stream, which _exit() made this stream wait for)
+      starts[:old['starts'].shape[0]].copy_(old['starts'])
+    for v in (starts, notes):  # read and written by the env's stream: not reused by torch before that stream is done
+      v.record_stream(self._stream)
+    _cabi.check(self._lib.cr_set_level_starts(self._handle, starts.data_ptr(), notes.data_ptr(), rows))
+    self._starts = dict(starts=starts, notes=notes)
+
+  def set_level_starts(self, starts):
+    """Give level table entries player starts (semantics: include/crafter_b200.h, cr_set_level_starts): an episode
+    drawn from or pinned to entry i whose record is on starts with the player at the record's (x, y), facing its
+    way, with its inventory (health, food, drink and energy included) and both last healths at its health; nothing
+    else about the fresh episode changes, and the world is still the one generated or authored for a start at the
+    centre.  A record that is off (all zeros) is the reference's start.  So a task curriculum can start deep goals
+    with their prerequisites (a stone pickaxe for collect_iron), and a probe is an authored world, a pinned env and a
+    start.
+
+    starts  (n, 20) ints, one record per table entry (see level_start), or a list of n items that are each None (the
+            reference's start), a dict of level_start keyword arguments (area: this env's), or a record; or None: no
+            starts.
+    A device int tensor is only checked for dtype and shape and is not read back (nothing synchronises); the device
+    decides whether a record is applicable when it installs an episode: the cell (x, y) must be grass, sand or path
+    and hold no creature, the rest as level_start checks it.  A record that is on but not applicable starts that
+    episode at the reference's start and raises error bit 8 (error_flags, check_errors).  Host input is checked
+    (ValueError).
+
+    An episode's start is fixed when its world seed is decided, like its goal: a rewritten start reaches an env from
+    its third new episode at the latest, and from the next one after sample_levels / pin_levels.  The start table
+    grows with the level table (new entries: 0).  Level -1 and fixed-level episodes start at the reference's start."""
+    if starts is None:
+      if self._starts is not None:
+        _cabi.check(self._lib.cr_set_level_starts(self._handle, None, None, 0))
+        self._starts = None
+      return
+    if self._table is None:
+      raise RuntimeError('set_level_starts: no level table (call set_level_table first)')
+    n = self._table_len
+    if torch.is_tensor(starts) or isinstance(starts, np.ndarray):
+      dtype = starts.dtype
+      if (dtype.is_floating_point or dtype.is_complex or dtype == torch.bool) if torch.is_tensor(starts) else (
+          dtype.kind not in 'iu'):
+        raise ValueError(f'starts must be integers, not {dtype}')
+      arr = starts.to(torch.int64) if torch.is_tensor(starts) else torch.from_numpy(starts.astype(np.int64))
+      if not arr.is_cuda:
+        if tuple(arr.shape) == (n, START_WORDS):
+          _check_starts(arr.numpy(), self._area)
+    else:
+      rows = []
+      for i, item in enumerate(starts):
+        if item is None:
+          rows.append(np.zeros(START_WORDS, np.int64))
+        elif isinstance(item, dict):
+          rows.append(level_start(**dict(dict(area=self._area), **item)))
+        else:
+          row = np.asarray(item)
+          if row.dtype.kind not in 'iu' or row.shape != (START_WORDS,):
+            raise ValueError(f'start {i} must be None, a dict of level_start arguments or {START_WORDS} ints')
+          rows.append(row)
+      arr = torch.from_numpy(np.array(rows, np.int64).reshape(-1, START_WORDS))
+      _check_starts(arr.numpy(), self._area)
+    if tuple(arr.shape) != (n, START_WORDS):
+      raise ValueError(f'starts must have shape ({n}, {START_WORDS}), not {tuple(arr.shape)}')
+    with torch.cuda.device(self._device):
+      if self._starts is None:
+        self._register_level_starts()
+      self._starts['starts'][:n].copy_(arr.to(self._device))
+
+  @property
+  def level_starts(self):
+    """A copy of the start records of the n table entries in use, int32 (n, 20), or None without starts."""
+    if self._starts is None:
+      return None
+    return self._starts['starts'][:self._table_len].clone()
 
   # ---- authored levels and pinning ----------------------------------------------------------------
   def _entries(self, entries, name, count=None):
@@ -1175,7 +1317,9 @@ class Env:
   def error_flags(self):
     """OR of the envs' sticky error bits (synchronises): 1 = an object was dropped because the slot
     arena was full (raise slot_capacity), 2 = an env was stepped past its daylight table, 4 = a sampled env
-    was seeded from an empty level table (no table, or a total weight of 0)."""
+    was seeded from an empty level table (no table, or a total weight of 0), 8 = an episode's level start was on but
+    not applicable (its cell not grass, sand or path, or holding a creature; see set_level_starts) and the episode
+    started at the reference's start."""
     flags = ctypes.c_int32(0)
     s = self._enter()
     _cabi.check(self._lib.cr_error_flags(self._handle, ctypes.byref(flags), s))
@@ -1195,6 +1339,11 @@ class Env:
     if flags & 4:
       raise RuntimeError('crafter_b200: a sampled env was seeded from an empty level table (total weight 0, or '
                          'no table); it played the world of the reference sequence instead')
+    if flags & ERR_LEVEL_START:
+      bad = self._state['pstate'][:, 14].bitwise_and(ERR_LEVEL_START).nonzero().flatten().tolist()
+      raise RuntimeError(f'crafter_b200: a level start was not applicable in envs {bad[:8]}{"..." if len(bad) > 8 else ""} '
+                         '(its cell is not grass, sand or path, or holds a creature, or the record is out of range); '
+                         "those episodes started at the reference's start")
 
   def set_inventory(self, values, env_ids=None):
     """Overwrite inventory entries ({item: amount}), like poking `env._player.inventory` on the
@@ -1220,13 +1369,16 @@ class Env:
     its running episodes under the entries they were drawn from (set_level_stats).  They are opt-in so that
     snapshots of batches with and without a level table keep the same keys.  The level table, cache and statistics
     are not env state.  With level goals it adds 'level_goal', the goal notes (num_envs, 4), so that the running
-    episodes keep their goals; the goal table itself is not env state either."""
+    episodes keep their goals; the goal table itself is not env state either.  With level starts it adds
+    'level_start', the start notes (num_envs, 4, 20), so that the episodes already decided keep their starts."""
     torch.cuda.synchronize(self._device)
     sd = {k: v.clone() for k, v in self._state.items()}
     if level_entries and self._ring is not None:
       sd['level_entry'], sd['final_level_entry'] = self._ring['entry'].clone(), self._ring['final'].clone()
     if level_entries and self._goals is not None:
       sd['level_goal'] = self._goals['notes'].clone()
+    if level_entries and self._starts is not None:
+      sd['level_start'] = self._starts['notes'].clone()
     return sd
 
   def load_state_dict(self, sd):
@@ -1237,6 +1389,7 @@ class Env:
       sd['final_world_seed'] = torch.zeros_like(self._state['final_world_seed'])
     ring = {k: sd.pop(key) for k, key in (('entry', 'level_entry'), ('final', 'final_level_entry')) if key in sd}
     notes = sd.pop('level_goal', None)
+    start_notes = sd.pop('level_start', None)
     if set(sd) != set(self._state):
       raise ValueError(f'state_dict of another layout (keys differ: {sorted(set(sd) ^ set(self._state))})')
     torch.cuda.synchronize(self._device)
@@ -1257,6 +1410,13 @@ class Env:
         self._goals['notes'].copy_(notes)
       else:
         self._goals['notes'].fill_(0)
+    if start_notes is not None and self._starts is None:  # start notes into a batch without starts: a table of zeros
+      self.set_level_starts(torch.zeros(self._table_len, START_WORDS, dtype=torch.int32, device=self._device))
+    if self._starts is not None:  # snapshots without start notes: their decided episodes start at the reference's
+      if start_notes is not None:
+        self._starts['notes'].copy_(start_notes)
+      else:
+        self._starts['notes'].fill_(0)
     self._needs_reset = False
 
   def recount(self):

@@ -31,7 +31,7 @@ class ShardedEnv:
   the same call: a child is a function of its parent's world, the key, its entry, the edits and the weights alone,
   so no bytes need to be broadcast.  level_stats gives the LOCAL shard's counts; they are integers, so their sum
   over the ranks (an all-reduce) is exactly what one big batch counts.  set_level_goals takes the same goals on
-every rank."""
+  every rank, and set_level_starts, like the goals, the same starts on every rank."""
 
   def __init__(self, num_envs, seed=0, env_factory=None, **kwargs):
     self.rank = dist.get_rank() if dist.is_initialized() else int(os.environ.get('RANK', 0))

@@ -192,6 +192,15 @@ class VectorEnv(_Base):
     """Env.level_goals: a copy of the goal masks of the table entries in use, or None."""
     return self.env.level_goals
 
+  def set_level_starts(self, starts):
+    """Env.set_level_starts: the player's start position, facing, inventory and vitals per level table entry."""
+    self.env.set_level_starts(starts)
+
+  @property
+  def level_starts(self):
+    """Env.level_starts: a copy of the start records of the table entries in use, or None."""
+    return self.env.level_starts
+
   def step(self, actions):
     obs, reward, done, info = self.env.step(actions)
     dead = self.env.state['final_stats'][:, 23] != 0

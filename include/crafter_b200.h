@@ -292,7 +292,8 @@ int cr_fill_level_cache(cr_handle *h, int first, int count, void *stream);
  * An entry i is authored when its cache row holds a caller-made world.  Everything else about the episode is what
  * it is for the generated world of seeds[i]: every draw after the world is built (creature updates, balance, night
  * noise) is keyed by seeds[i], PS_WORLD_SEED and final_world_seed report seeds[i], and the player starts at
- * (W/2, H/2) with the reference's fresh vitals and inventory.  So an authored episode is a function of (authored
+ * (W/2, H/2) with the reference's fresh vitals and inventory unless the entry has a level start
+ * (cr_set_level_starts).  So an authored episode is a function of (authored
  * world, seeds[i], actions) and replays bit for bit from those three.  The copy rule of the cache does not change:
  * a row is installed when its tag equals the drawn seed.  cr_author_levels tags a row with seeds[i] as the table
  * holds it when the row is written, so an authored row survives cr_fill_level_cache while its entry keeps that
@@ -442,6 +443,47 @@ int cr_set_level_stats(cr_handle *h, int32_t *entry, int32_t *final_entry, int64
  * cr_set_level_stats it changes pointers only (the cached step graphs are captured again at the next step). */
 int cr_set_level_goals(cr_handle *h, const int32_t *goals, int32_t *notes, int cap);
 
+/* Level starts: a level table entry can set where its episodes' player starts, facing which way, holding what, with
+ * which vitals.  So a task curriculum can start deep goals with their prerequisites in hand (a stone pickaxe for
+ * collect_iron), and an evaluation probe is an authored world, a pinned env and a start.
+ *
+ * Start table: `starts` int32[cap][CR_START_WORDS]; row i is entry i's start:
+ *   word 0      on: 0 is the reference's start (the other words are ignored), so an all-zero table is the reference
+ *   words 1-2   the player's x and y
+ *   word 3      the facing: 0 left, 1 right, 2 up, 3 down (the facing index of the player's slot record)
+ *   words 4-19  the inventory in data.yaml order, health first
+ *
+ * When a start is fixed: `notes` int32[num_envs][4][CR_START_WORDS] is a ring indexed by episode & 3, like the goal
+ * notes.  Whenever the world seed of episode e of an env is decided, slot e & 3 gets a copy of starts[r] for the entry
+ * r it was drawn from or pinned to, when r < cap; otherwise a row of zeros (level -1, a fixed level, an empty table, a
+ * pinned entry at or beyond *n, an entry at or beyond the starts' capacity).  cr_set_levels, cr_sample_levels and
+ * cr_pin_levels decide e + 1 and e + 2 again and note them again; the running episode keeps its start.  So a rewritten
+ * start has the goals' staleness: it reaches an env from its third new episode at the latest, and from the next one
+ * after cr_sample_levels / cr_pin_levels.
+ *
+ * Applied when episode e is installed, from note e & 3.  A record that is on is applicable when 0 <= x < W,
+ * 0 <= y < H, the facing lies in 0..3, every item lies in [0, 9] with health in [1, 9], and the installed world's cell
+ * (x, y) is grass, sand or path and holds no creature.  Then the fresh player is the reference's Player(world, (x, y))
+ * with that facing and inventory: its slot is 1 and its object-map cell is (x, y); the touched chunk is the chunk of
+ * (x, y); both last healths (PS_P_LAST_HEALTH, PS_LAST_HEALTH) are the start's health, so the first step pays no
+ * health delta; achievements, PS_UNLOCKED, sleeping and the hidden counters (hunger, thirst, fatigue, recover) are 0
+ * as in every fresh episode.  A record that is on but not applicable gives the reference's start for the whole
+ * episode and raises the env's sticky error bit 3 (value 8, see cr_error_flags).
+ *
+ * The start does not change the world: a generated world is still generated for a player at (W/2, H/2) (the creature
+ * distances and the start clearing), cr_author_levels still checks the centre cell, and cr_mutate_levels still never
+ * edits the centre (it may edit a custom start cell).  Only where the player stands moves.
+ *
+ * An episode is a function of (world, seeds[i], goal, start, actions).  A batch with starts registered, every `on`
+ * 0, equals bit for bit the same batch without starts, in every output and in all of cr_state.
+ *
+ * cr_set_level_starts registers caller-owned DEVICE buffers, valid until replaced, removed or cr_destroy: starts ==
+ * NULL removes both.  The caller rewrites `starts` with stream-ordered writes whenever it likes.  Fails when starts is
+ * given without notes or with cap < 1.  No stream: like cr_set_level_goals it changes pointers only (the cached step
+ * graphs are captured again at the next step). */
+#define CR_START_WORDS 20
+int cr_set_level_starts(cr_handle *h, const int32_t *starts, int32_t *notes, int cap);
+
 /* After the caller has written `mat` itself (state restore, tests): recount what the library keeps
  * incrementally about the terrain (the per-chunk counts of chunk_cnt; a no-op without that buffer
  * or with CRAFTER_B200_INCR_CENSUS=0). */
@@ -450,7 +492,9 @@ int cr_recount(cr_handle *h, void *stream);
 /* OR of the envs' sticky error bits (pstate column 14) into *flags_host, synchronising the stream:
  * bit 0 an object did not fit the slot arena and was dropped (raise slot_capacity), bit 1 an env's step
  * counter ran past the daylight table (n_daylight entries; the last one is used from there on), bit 2 a sampled
- * env was seeded from an empty level table (cr_set_level_table) and plays the reference sequence's world. */
+ * env was seeded from an empty level table (cr_set_level_table) and plays the reference sequence's world, bit 3 an
+ * installed episode's level start was on but not applicable and the episode started at the reference's start
+ * (cr_set_level_starts). */
 int cr_error_flags(cr_handle *h, int32_t *flags_host, void *stream);
 
 /* Number of kernel launches issued by this handle so far (bench.py's gpu_launches). */
