@@ -26,8 +26,9 @@ constexpr int UPDATE_WPB = CR_UPDATE_WPB;  // warps (= envs) per CTA of k_update
 constexpr int SEED_WPB = 4;
 constexpr int RENDER_THREADS = RENDER_NT;
 #ifndef CR_RENDER_MIN_CTAS
-#define CR_RENDER_MIN_CTAS (RENDER_NT <= 128 ? 8 : DEF ? 4 : 2)  // sm_90a, default geometry: 64 registers, no
-// spills (H100 SXM 80 GB at 700 W: 134 vs 150 us/step at 6 CTAs / 40 registers, which spill); the generic
+#define CR_RENDER_MIN_CTAS (RENDER_NT <= 128 ? 8 : DEF ? 5 : 2)  // sm_90a, default geometry: 48 registers, no
+// spills, since the whole CTA gathers the view window (warp 0 alone held 8 cells' loads per lane: 64 registers =
+// 4 CTAs, and 40 registers spilled).  H100 SXM 80 GB at 700 W: 32.1 vs 30.6 M env-steps/s at 4 CTAs.  The generic
 // instantiation spills below 2 CTAs' 128 registers (its larger frames are bound by shared memory anyway)
 #endif
 #ifndef CR_WG_THREADS
@@ -558,7 +559,7 @@ __global__ void __launch_bounds__(VIEW_WPB * 32) k_view(Geom g, State st, Render
   if (threadIdx.x == 0 && blockIdx.x < 1024) cr_stamp(4096 + 3072 + (int)blockIdx.x, 0);  // profiling aid
   if (env >= g.B || !(st.frame_night[env] & FRAME_FINAL)) return;
   RenderView &V = sv[warp];
-  render_gather(g, st, rt, env, lane, V);
+  render_gather(g, st, env, lane, V);
   __syncwarp();
   const Word16 *src = reinterpret_cast<const Word16 *>(&V);
   Word16 *dst = reinterpret_cast<Word16 *>(st.frame_view) + (size_t)env * VIEW_WORDS;

@@ -118,8 +118,8 @@ CR_DEV uint32_t color_fx(const RenderShared &S, uint32_t c, uint32_t n, int slee
 }
 
 // ---- phases 1 + 2: stage and plan ---------------------------------------------------------------
-// Warp 0 gathers the view window (three dependent global loads per cell) and plans the tile jobs;
-// meanwhile the other warps build the FP64 / float tables.  One CTA barrier follows.
+// The view window (render_cells: three dependent global loads per cell) and one CTA barrier; then warp 0
+// plans the tile jobs while the other warps build the FP64 / float tables.  One CTA barrier follows.
 CR_DEV void render_plan(const Geom &g, RenderView &V, int lane);
 
 // The FP64 / float tables of the frame: threads CR_LANES.. of the CTA (they depend on the step's
@@ -138,64 +138,23 @@ CR_DEV void render_tables(int tid, int nthreads, RenderShared &S, double dayligh
   }
 }
 
-CR_DEV void render_gather(const Geom &g, const State &st, const RenderTables &rt, int env, int lane,
-                          RenderView &V);
-
-struct alignas(16) Word16 { uint64_t a, b; };
-constexpr int VIEW_WORDS = (int)(sizeof(RenderView) / 16);
-
-// `ahead`: the env's view and tile plan as k_view prepared them after the tick, valid when `*flag` says
-// FRAME_FINAL (null: gather here).  The copy is issued before the flag is looked at: one coalesced round
-// trip instead of three dependent ones.
-CR_DEV void render_stage(const Geom &g, const State &st, const RenderTables &rt, int env, int tid,
-                         int nthreads, RenderShared &S, double daylight, const RenderView *ahead = nullptr,
-                         const uint8_t *flag = nullptr) {
-  if (tid >= CR_LANES) {
-    render_tables(tid, nthreads, S, daylight);
-  } else if (ahead) {
-    constexpr int PER = (VIEW_WORDS + CR_LANES - 1) / CR_LANES;
-    const Word16 *src = reinterpret_cast<const Word16 *>(ahead);
-    Word16 *dst = reinterpret_cast<Word16 *>(&S.V);
-    Word16 w[PER];
-#pragma unroll
-    for (int q = 0; q < PER; ++q) {
-      const int i = tid + q * CR_LANES;
-      if (i < VIEW_WORDS) w[q] = src[i];
-    }
-    if (*flag & FRAME_FINAL) {  // uniform across the warp
-#pragma unroll
-      for (int q = 0; q < PER; ++q) {
-        const int i = tid + q * CR_LANES;
-        if (i < VIEW_WORDS) dst[i] = w[q];
-      }
-    } else {
-      render_gather(g, st, rt, env, tid, S.V);
-    }
-  } else {
-    render_gather(g, st, rt, env, tid, S.V);
-  }
-}
-
-// Warp 0: the view window (three dependent global loads per cell), then the tile plan.
-CR_DEV void render_gather(const Geom &g, const State &st, const RenderTables &rt, int env, int lane,
-                          RenderView &V) {
+// The view cells c0, c0 + stride, ... (N of them; cell = i * vh + j over the whole view, item rows included):
+// material id, sprite id and tile id.  All grid loads of the N cells are issued before any is consumed, then
+// all slot-record loads: three dependent round trips in total, not three per cell.
+template <int N>
+CR_DEV void render_cells(const Geom &g, const State &st, int env, int c0, int stride, RenderView &V) {
   const int32_t *ps = st.pstate + (size_t)env * PS_COUNT;
   const int px = ps[PS_PX], py = ps[PS_PY], sleeping = ps[PS_SLEEPING];
   const uint8_t *mat = st.mat + (size_t)env * g.NC;
   const uint16_t *objmap = st.objmap + (size_t)env * g.NC;
   const Ent *ents = st.ents + (size_t)env * g.CAP;
-  const int offx = g.gx / 2, offy = g.gy / 2;  // engine.py:161
   const int32_t *inv = st.inventory + (size_t)env * N_ITEMS;
-  for (int i = lane; i < N_ITEMS; i += CR_LANES) V.inv[i] = inv[i];
-  cr_syncwarp();
-  // cell = i * vh + j over the whole view.  All grid loads of a lane are issued before any is
-  // consumed, then all slot-record loads: three dependent round trips in total, not three per cell.
-  constexpr int MAXC = 256 / CR_LANES > 8 ? 256 : 8;  // cells per lane (8 on the device)
+  const int offx = g.gx / 2, offy = g.gy / 2;  // engine.py:161
   const int cells = g.vw * g.vh;
-  int gcell[MAXC], mm[MAXC], slot[MAXC];
+  int gcell[N], mm[N], slot[N];
 #pragma unroll
-  for (int q = 0; q < MAXC; ++q) {
-    const int c = lane + q * CR_LANES;
+  for (int q = 0; q < N; ++q) {
+    const int c = c0 + q * stride;
     gcell[q] = -1; mm[q] = 0; slot[q] = 0;
     if (c < cells) {
       const int i = c / g.vh, j = c - i * g.vh;
@@ -204,15 +163,15 @@ CR_DEV void render_gather(const Geom &g, const State &st, const RenderTables &rt
     }
   }
 #pragma unroll
-  for (int q = 0; q < MAXC; ++q)
+  for (int q = 0; q < N; ++q)
     if (gcell[q] >= 0) { mm[q] = mat[gcell[q]] & 0x7F; slot[q] = objmap[gcell[q]]; }
-  Ent er[MAXC];
+  Ent er[N];
 #pragma unroll
-  for (int q = 0; q < MAXC; ++q)
+  for (int q = 0; q < N; ++q)
     if (slot[q]) er[q] = ents[slot[q]];
 #pragma unroll
-  for (int q = 0; q < MAXC; ++q) {
-    const int c = lane + q * CR_LANES;
+  for (int q = 0; q < N; ++q) {
+    const int c = c0 + q * stride;
     if (c >= cells) continue;
     const int i = c / g.vh, j = c - i * g.vh;
     int tile = N_TILES, o = 255;
@@ -221,14 +180,67 @@ CR_DEV void render_gather(const Geom &g, const State &st, const RenderTables &rt
       if (slot[q]) o = sprite_of(er[q], sleeping);
     } else {  // item strip, engine.py:227-235: inventory order, vw per row; empty slots stay black
       const int index = (j - g.gy) * g.vw + i;
-      if (index < N_ITEMS && V.inv[index] >= 1) tile = TILE_ITEM0 + index;
+      if (index < N_ITEMS && inv[index] >= 1) tile = TILE_ITEM0 + index;
     }
     V.tmat[c] = (uint8_t)mm[q];
     V.tobj[c] = (uint8_t)o;
     V.tidx[c] = (uint8_t)tile;
   }
+}
+
+// One warp (k_view): the inventory and the view window, its lanes striding over the cells, then the tile plan.
+CR_DEV void render_gather(const Geom &g, const State &st, int env, int lane, RenderView &V) {
+  const int32_t *inv = st.inventory + (size_t)env * N_ITEMS;
+  for (int i = lane; i < N_ITEMS; i += CR_LANES) V.inv[i] = inv[i];
+  render_cells<256 / CR_LANES>(g, st, env, lane, CR_LANES, V);  // cr_create: at most 256 cells
   cr_syncwarp();
   render_plan(g, V, lane);
+}
+
+struct alignas(16) Word16 { uint64_t a, b; };
+constexpr int VIEW_WORDS = (int)(sizeof(RenderView) / 16);
+
+// `ahead`: the env's view and tile plan as k_view prepared them after the tick, valid when `*flag` says
+// FRAME_FINAL (null: gather here).  Warp 0 issues the copy before the flag is looked at: one coalesced round
+// trip instead of three dependent ones.  Otherwise the whole CTA gathers the window, one view cell per thread
+// (a CTA of one-lane warps runs its threads one after another: its thread 0 takes every cell), and the tile
+// plan waits for one more CTA barrier.
+CR_DEV void render_stage(const Geom &g, const State &st, const RenderTables &rt, int env, int tid,
+                         int nthreads, RenderShared &S, double daylight, const RenderView *ahead = nullptr,
+                         const uint8_t *flag = nullptr) {
+  (void)rt;
+  constexpr int PER = (VIEW_WORDS + CR_LANES - 1) / CR_LANES;
+  Word16 w[PER];
+  if (ahead && tid < CR_LANES) {
+    const Word16 *src = reinterpret_cast<const Word16 *>(ahead);
+#pragma unroll
+    for (int q = 0; q < PER; ++q) {
+      const int i = tid + q * CR_LANES;
+      if (i < VIEW_WORDS) w[q] = src[i];
+    }
+  }
+  const bool gather = !ahead || !(*flag & FRAME_FINAL);  // uniform across the CTA
+  if (gather) {
+    const int gt = CR_LANES == 1 ? 1 : nthreads;
+    if (tid < gt) {
+      const int32_t *inv = st.inventory + (size_t)env * N_ITEMS;
+      for (int i = tid; i < N_ITEMS; i += gt) S.V.inv[i] = inv[i];
+      for (int c = tid; c < g.vw * g.vh; c += gt) render_cells<1>(g, st, env, c, 0, S.V);
+    }
+    cr_syncblock();
+  }
+  if (tid >= CR_LANES) {
+    render_tables(tid, nthreads, S, daylight);
+  } else if (gather) {
+    render_plan(g, S.V, tid);
+  } else {
+    Word16 *dst = reinterpret_cast<Word16 *>(&S.V);
+#pragma unroll
+    for (int q = 0; q < PER; ++q) {
+      const int i = tid + q * CR_LANES;
+      if (i < VIEW_WORDS) dst[i] = w[q];
+    }
+  }
 }
 
 // Which tiles does this frame need?  Materials present in the window, one tile per visible object
